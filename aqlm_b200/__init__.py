@@ -1,4 +1,4 @@
-"""aqlm_b200 -- B200-native (sm_100a) implementation of AQLM's quantized-linear hot path.
+"""aqlm_b200 -- H100-native (sm_90a) implementation of AQLM's quantized-linear hot path.
 
 Mirrors the reference `aqlm` package surface (inference_lib/src/aqlm/__init__.py:1-3): `QuantizedLinear`,
 `inference_kernels.{get_forward_pass_kernel,get_backward_pass_kernel,optimize_for_training}`, `utils.*`.

@@ -1,7 +1,7 @@
 """ctypes binding of the aqlm_b200 C-ABI (include/aqlm_b200.h) + the in-tree nvcc build.
 
 PyTorch is plumbing here (device memory, streams); the product is `csrc/libaqlm_b200.so`.  There is no
-CPU fallback: if the library is missing or the device is not sm_100, every op raises.
+CPU fallback: if the library is missing or the device is not sm_90, every op raises.
 """
 from __future__ import annotations
 
@@ -17,7 +17,7 @@ LIB_PATH = os.environ.get("AQLM_B200_LIB") or os.path.join(CSRC, "libaqlm_b200.s
 HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "aqlm_b200.h")
 SOURCES = ["capi.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 
@@ -51,7 +51,7 @@ def _stale() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/*.cu for sm_100a into csrc/libaqlm_b200.so (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/*.cu for sm_90a into csrc/libaqlm_b200.so (nvcc cross-compiles without a GPU)."""
     if force or _stale():
         cmd = ["nvcc", *NVCC_FLAGS, "-o", LIB_PATH, *[os.path.join(CSRC, s) for s in SOURCES]]
         if verbose:

@@ -7,8 +7,8 @@
 
 #include "common.cuh"
 #include "dequant.cuh"
-#include "gemm_tcgen05.cuh"
-#include "gemm_tcgen05_t.cuh"
+#include "gemm_wgmma.cuh"
+#include "gemm_wgmma_t.cuh"
 #include "gemv.cuh"
 #include "gemv_lut.cuh"
 #include "peer_allreduce.cuh"
@@ -41,8 +41,8 @@ const DeviceInfo* device_info() {
       d.ok = true;
     }
   }
-  if (d.cc_major != 10) {
-    fail(AQLM_B200_ERR_ARCH, "aqlm_b200 is built for sm_100a only; device %d is sm_%d%d", dev, d.cc_major, d.cc_minor);
+  if (d.cc_major != 9 || d.cc_minor != 0) {
+    fail(AQLM_B200_ERR_ARCH, "aqlm_b200 is built for sm_90a only; device %d is sm_%d%d", dev, d.cc_major, d.cc_minor);
     return nullptr;
   }
   return &d;
@@ -58,7 +58,7 @@ static int env_int(const char* name, int dflt) {
 struct Tunables {
   int pdl, gemv_ctas_per_sm, gemv_threads, gather_mode, gemv_v2, force_generic;
   int disable_lut, lut_ctas_per_sm, lut_debug, lut_cluster, lut_batch_loop, lut_rb16, lut_c2_rb;
-  int disable_tcgen05, gemm_stages, gemm_ksplit, gemm_cluster, gemm_debug, gemm_gather_mode, gemm_v2, gemm_tile_m, gemm_atmem, gemm_a_stages, gemm_groups;
+  int disable_wgmma, gemm_stages, gemm_ksplit, gemm_gather_mode, gemm_tile_m;
   void load() {
     pdl = env_int("AQLM_B200_PDL", 1);
     gemv_ctas_per_sm = env_int("AQLM_B200_GEMV_CTAS_PER_SM", 1);
@@ -71,25 +71,18 @@ struct Tunables {
     lut_debug = env_int("AQLM_B200_LUT_DEBUG", 0);
     lut_batch_loop = env_int("AQLM_B200_LUT_BATCH_LOOP", 1);  // batch 2-3 on 256-entry codebooks: one LUT launch per row
     lut_rb16 = env_int("AQLM_B200_LUT_RB16", 0);  // cluster kernel: 16-row warp batches on 768 threads (experiment)
-    lut_c2_rb = env_int("AQLM_B200_LUT_C2_RB", 0);  // cluster kernel, second form: rows per warp batch (0: by row-block size; 16; 32)
+    lut_c2_rb = env_int("AQLM_B200_LUT_C2_RB", 0);  // cluster kernel, second form: rows per warp batch (0: 16; 16; 32)
     // K <= 2, in <= 4096: slab CTAs form a cluster, DSMEM reduction.  0: off (workspace kernel), 1: first form, 2: second form,
-    // 3 (default): second form for row blocks of <= 768 rows = at most 24 warps of 32 rows, the 768-thread / 80-register
-    // build (Llama-2-7B: 4096 -> 4096 / 11008; 15 clusters of 8 CTAs were resident on the measured boxes, i.e. blocks of
-    // 288 and 736 rows), first form above, where the second form needs its 1024-thread / 64-register build and spills
-    // (measured, profiles/r02/probe_lut2_n.jsonl: second form +12..+27 % up to 11008 rows, -2..-4 % at 12288 / 22016
-    // rows = blocks of 832 / 1472 rows)
+    // 3 (default, automatic): the second form with 16-row warp batches at every row-block size.  Measured with
+    // tools/probe_lut2.py on an H100 80GB HBM3 (400 W limit): fastest or tied on every probed shape, e.g. 2x8 4096 -> 11008 /
+    // 12288 / 22016 in 12.1 / 12.6 / 17.9 us against 13.7 / 15.3 / 24.4 us for the first form and 14.4 / 17.1 / 26.9 us
+    // for 32-row batches.
     lut_cluster = env_int("AQLM_B200_LUT_CLUSTER", 3);
-    disable_tcgen05 = env_int("AQLM_B200_DISABLE_TCGEN05", 0);
+    disable_wgmma = env_int("AQLM_B200_DISABLE_WGMMA", 0);
     gemm_stages = env_int("AQLM_B200_GEMM_STAGES", 0);
     gemm_ksplit = env_int("AQLM_B200_GEMM_KSPLIT", 0);
-    gemm_cluster = env_int("AQLM_B200_GEMM_CLUSTER", 0);  // 0: per plan (pairs of CTAs multicast the X tile: 52.7 vs 55.1 us at 4096->14336 bs=256; 4 is slower)
-    gemm_debug = env_int("AQLM_B200_GEMM_DEBUG", 0);
     gemm_gather_mode = env_int("AQLM_B200_GEMM_GATHER_MODE", -1);  // -1: per scheme (1x16: ld.global.cg, no L1 allocation of the 1 MiB codebook's lines; 256-entry codebooks: L1-resident)
-    gemm_v2 = env_int("AQLM_B200_GEMM_V2", -1);                   // -1: per-scheme default
     gemm_tile_m = env_int("AQLM_B200_GEMM_TILE_M", 0);            // 0: chosen by the plan
-    gemm_a_stages = env_int("AQLM_B200_GEMM_A_STAGES", 0);        // ATMEM: A stages in tensor memory (0: 6)
-    gemm_groups = env_int("AQLM_B200_GEMM_GROUPS", 0);            // ATMEM: producer groups of 4 warps (0: 3, max 4)
-    gemm_atmem = env_int("AQLM_B200_GEMM_ATMEM", -1);             // A operand in tensor memory; -1: per-scheme default
   }
 };
 static Tunables& tun() {
@@ -521,8 +514,8 @@ static int launch_lut_cluster(const aqlm_b200_weight_t* w, const void* input, vo
   rpb = (rpb + 31) / 32 * 32;
   if (rpb > 2048) return AQLM_B200_OK;  // per-row partials live in shared memory
   const int row_blocks = (int)((w->out_features + rpb - 1) / rpb);
-  if (tun().lut_cluster == 2 || (tun().lut_cluster >= 3 && rpb <= 768)) {  // second form: same grid / cluster shape, its own CTA size and shared-memory map
-    const int rb_sel = tun().lut_c2_rb ? tun().lut_c2_rb : (rpb <= 512 ? 16 : 32);
+  if (tun().lut_cluster >= 2) {  // second form: same grid / cluster shape, its own CTA size and shared-memory map
+    const int rb_sel = tun().lut_c2_rb ? tun().lut_c2_rb : 16;
     const int rc = rb_sel == 16 ? launch_lut_cluster2<T, K, 16>(w, input, output, flags, di, st, rpb, row_blocks, n_slabs)
                                 : launch_lut_cluster2<T, K, 32>(w, input, output, flags, di, st, rpb, row_blocks, n_slabs);
     *taken = rc == AQLM_B200_OK;
@@ -571,7 +564,7 @@ static int try_lut_cluster(const aqlm_b200_weight_t* w, const void* input, void*
 #undef AQLM_LUTC
 }
 
-// ---- fused dequant + tcgen05 GEMM: host side ------------------------------------------------------
+// ---- fused dequant + wgmma GEMM: host side ------------------------------------------------------
 typedef CUresult (*tmap_encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -601,14 +594,31 @@ static void ensure_driver_context() {
 
 
 struct GemmPlan {
-  bool ok = false;       // tcgen05 path applicable
-  int m_tiles = 0, n_tiles = 0, n_tile = 0, ksplit = 1, stages = 0, total_kblocks = 0, cluster = 1;
+  bool ok = false;       // tensor-core (wgmma) path applicable
+  int m_tiles = 0, n_tiles = 0, n_tile = 0, ksplit = 1, stages = 0, total_kblocks = 0;
   int tile_m = kGemmBlockM;  // output rows per CTA tile
-  bool v2 = false;           // producer mapping: one 4-warp group per stage, thread <-> row
-  bool atmem = false;        // A operand written to tensor memory (needs v2)
-  int a_stages = 0, groups = 0;  // ATMEM: A stages in TMEM (decoupled from the X stages) / V2: producer groups
   size_t counters_bytes = 0, partials_bytes = 0;
 };
+
+// MMA width: the smallest wgmma N of {16, 32, 64, 128} covering the batch (larger batches: tiles of 128)
+static void gemm_n_tiles(int64_t batch, int* n_tile, int* n_tiles) {
+  int n = 16;
+  while (n < kGemmMaxN && n < batch) n <<= 1;
+  *n_tile = n;
+  *n_tiles = (int)((batch + n - 1) / n);
+}
+
+// Cost of one k-block of one CTA in SM clocks: max(gathers, tensor pipe, shared-memory traffic) + a fixed
+// synchronisation cost.  Model constants, not measurements: gathers of 16-byte codebook vectors at ~0.6 per clock from
+// L2 (the 1 MiB 1x16 codebook) and ~1.1 from L1 (256-entry codebooks); the tensor pipe at 2048 fp16 MACs per clock
+// per SM (the data-sheet dense rate); shared memory at 128 bytes per clock.
+static double gemm_kblock_clk(int rows, int K, int nbits, int n_tile, double smem_bytes) {
+  const double t_gather = rows * 8.0 * K / (nbits == 16 ? 0.6 : 1.1);
+  const double t_mma = 128.0 * n_tile * 64.0 / 2048.0;
+  const double t_smem = smem_bytes / 128.0;
+  double t = t_gather > t_mma ? t_gather : t_mma;
+  return (t > t_smem ? t : t_smem) + 60.0;
+}
 
 static GemmPlan gemm_plan(const aqlm_b200_weight_t* w, int64_t batch, const DeviceInfo* di, bool allow_split) {
   GemmPlan g;
@@ -621,68 +631,34 @@ static GemmPlan gemm_plan(const aqlm_b200_weight_t* w, int64_t batch, const Devi
   // TMA needs a 16-byte multiple as the global row stride of the code matrix (1x8: in_features % 128 == 0);
   // other shapes take the GEMV fallback in aqlm_b200_matmat_dequant_ws
   if (((size_t)(w->in_features / 8) * K * cb) % 16 != 0) return g;
-  if (tun().disable_tcgen05) return g;
+  if (tun().disable_wgmma) return g;
   g.total_kblocks = (int)(w->in_features / kGemmBlockK);
-  if (batch <= 256) {
-    g.n_tile = (int)((batch + 15) / 16 * 16);
-    g.n_tiles = 1;
-  } else {
-    g.n_tile = 256;
-    g.n_tiles = (int)((batch + 255) / 256);
-  }
-  // producer mapping V2 (one 4-warp group per stage) measured: 1x16 496 vs 505 TFLOP/s (V1), 2x8 134 vs 394, 8x8 196 vs 119
-  // -> V2 for schemes with many codebooks; A-in-TMEM builds on V2 (profiles/r01/gemm_experiments.md, profiles/r02/)
-  // A in tensor memory: measured 1x16 61.7 -> 55.1 us, 2x8 69.3 -> 49.2 us (4096->14336/11008, bs=256); 8x8 no gain
-  g.atmem = (tun().gemm_atmem < 0 ? (K <= 2) : tun().gemm_atmem != 0) && !(tun().gemm_debug & 1);
-  g.v2 = g.atmem || ((tun().gemm_v2 < 0 ? (K >= 4 ? 1 : 0) : tun().gemm_v2) != 0 && !(tun().gemm_debug & 1));
+  gemm_n_tiles(batch, &g.n_tile, &g.n_tiles);
   const size_t budget = (size_t)di->max_smem_optin;
-  // At most 3 stages: shared memory taken here is L1 taken from the codebook gathers (outstanding misses need L1
-  // lines); measured at N=256: 4 stages 335 TFLOP/s, 3 stages 484-503, 2 stages 470 (profiles/r01/gemm_experiments.md)
+  // At most 3 stages: shared memory taken here is L1 taken from the codebook gathers (outstanding misses need L1 lines)
   int S = 3;
-  while (S > 2 && gemm_smem_layout(S, g.n_tile, g.atmem).total > budget) --S;
-  if (gemm_smem_layout(S, g.n_tile, g.atmem).total > budget) return g;
+  while (S > 2 && gemm_smem_layout(S, g.n_tile).total > budget) --S;
+  if (gemm_smem_layout(S, g.n_tile).total > budget) return g;
   const int forced_s = tun().gemm_stages;
-  if (forced_s >= 2 && forced_s <= S) S = forced_s;
-  if (forced_s == 4 && g.v2 && gemm_smem_layout(4, g.n_tile, g.atmem).total <= budget) S = 4;  // experiment: 4 X stages
+  if (forced_s >= 2 && forced_s <= 4 && gemm_smem_layout(forced_s, g.n_tile).total <= budget) S = forced_s;
   g.stages = S;
-  g.groups = S;
-  g.a_stages = S;
-  if (g.atmem) {
-    // tensor memory: accumulator columns [0, n_tile), then 32 columns per A stage; 512 columns in all
-    const int room = (512 - ((g.n_tile + 31) & ~31)) / 32;
-    int sa = tun().gemm_a_stages > 0 ? tun().gemm_a_stages : 6;
-    if (sa > room) sa = room;
-    if (sa > 8) sa = 8;
-    if (sa < 2) sa = 2;
-    g.a_stages = sa;
-    g.groups = tun().gemm_groups > 0 ? (tun().gemm_groups > 4 ? 4 : tun().gemm_groups) : 3;
-  }
   // ---- tile height and split-K: a small cost model over (tile_m, ksplit), in SM clocks ----
-  //   per k-block of one CTA: max(gathers, tensor pipe, shared-memory traffic) + a fixed synchronisation cost;
-  //   per CTA: its k-blocks + a fixed cost (launch ramp, TMEM alloc, pipeline fill, epilogue: ~5 us measured);
+  //   per CTA: its k-blocks + a fixed cost (launch ramp, pipeline fill, epilogue: ~5 us);
   //   per launch: waves x CTA time + split-K fix-up traffic (partials written and read once through L2).
-  // The gather rate is the measured per-SM rate of random 16-byte codebook reads (profiles/: ~0.85/clk from L2 for the
-  // 1 MiB 1x16 codebook; 256-entry codebooks are L1-resident and gather faster).
-  const double clk = 1.9e9;
-  const double gather_per_clk = (nbits == 16 ? 0.85 : 1.6) * (g.atmem ? 1.0 : 0.7);  // SS form: smaller L1 -> slower gathers
-  const double t_mma = 2.0 * g.n_tile;                                                 // 4 x (128 x N x 16) at 4096 MAC/clk
+  const double clk = 1.7e9;
   int best_tm = kGemmBlockM, best_ks = 1;
   double best = 1e30;
   const int max_ks = !allow_split ? 1 : (g.total_kblocks / 2 < 16 ? (g.total_kblocks / 2 < 1 ? 1 : g.total_kblocks / 2) : 16);
-  const bool want_pairs = (tun().gemm_cluster > 0 ? tun().gemm_cluster : (g.n_tile >= 128 ? 2 : 1)) > 1;
   for (int tm = kGemmBlockM; tm >= 32; tm -= (tm > 64 ? 1 : 8)) {
     const long long tiles = ((w->out_features + tm - 1) / tm) * (long long)g.n_tiles;
     if (tiles > kGemmMaxTiles) continue;
-    // CTA pairs multicast the X tile: keep the number of M tiles even (full-height tiles stay as the fallback)
-    if (want_pairs && tm != kGemmBlockM && (((w->out_features + tm - 1) / tm) & 1)) continue;
-    const double t_gather = tm * 8.0 * K / gather_per_clk;
-    const double t_smem = (g.atmem ? 0.0 : (128.0 + tm) * 128.0 / 128.0) + 2.0 * g.n_tile;  // bytes / (128 B/clk)
-    const double t_kb = (t_gather > t_mma ? (t_gather > t_smem ? t_gather : t_smem) : (t_mma > t_smem ? t_mma : t_smem)) + 60.0;
+    // smem bytes per k-block: A written once and read once, B written once and read by both consumer warpgroups
+    const double t_kb = gemm_kblock_clk(tm, K, nbits, g.n_tile, 2.0 * 128 * 128 + 3.0 * g.n_tile * 128);
     for (int c = 1; c <= max_ks; ++c) {
       const double ctas = (double)tiles * c;
       const double waves = (double)((long long)((ctas + di->sm_count - 1) / di->sm_count));
       const double kb_cta = (double)((g.total_kblocks + c - 1) / c);
-      const double fix = c > 1 ? ctas * g.n_tile * kGemmBlockM * 4.0 * 2.0 / 4e12 * clk : 0.0;
+      const double fix = c > 1 ? ctas * g.n_tile * kGemmBlockM * 4.0 * 2.0 / 3e12 * clk : 0.0;
       const double t = waves * (kb_cta * t_kb + 5e-6 * clk) + fix;
       if (t < best * (tm == kGemmBlockM && c == 1 ? 1.0 : 0.97)) {  // prefer full tiles / fewer splits unless the gain is real
         best = t;
@@ -703,14 +679,31 @@ static GemmPlan gemm_plan(const aqlm_b200_weight_t* w, int64_t batch, const Devi
   g.counters_bytes = kWsCountersBytes;
   if ((size_t)g.m_tiles * g.n_tiles > (size_t)kGemmMaxTiles) ks = 1;
   g.ksplit = ks;
-  // X-tile multicast: CTAs of a cluster (consecutive M tiles, same K range) each TMA-load 1/C of the X tile and
-  // multicast it to all C, cutting the L2->SM traffic of X by C.
-  int cl = tun().gemm_cluster > 0 ? tun().gemm_cluster : (g.n_tile >= 128 ? 2 : 1);
-  while (cl > 1 && (g.m_tiles % cl != 0 || g.n_tile % (8 * cl) != 0)) cl >>= 1;
-  g.cluster = cl < 1 ? 1 : cl;
   g.partials_bytes = ks > 1 ? (size_t)g.m_tiles * g.n_tiles * ks * g.n_tile * kGemmBlockM * 4 : 0;
   g.ok = true;
   return g;
+}
+
+template <typename T, int K, int CB, int N>
+static int launch_gemm_n(const CUtensorMap& tx, const CUtensorMap& tc, const GemmParams& p, const GemmPlan& g,
+                         const DeviceInfo* di, cudaStream_t st) {
+  const size_t smem = gemm_smem_layout(g.stages, N).total;
+  auto kernel = gemm_dequant_kernel<T, K, CB, N>;
+  static SmemMarks marks;
+  if (int rc = ensure_smem(kernel, smem, marks, di)) return rc;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(g.m_tiles, g.ksplit, g.n_tiles);
+  cfg.blockDim = dim3(kGemmThreads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = tun().pdl ? 1 : 0;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  AQLM_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, tx, tc, p));
+  count_launch();
+  return AQLM_B200_OK;
 }
 
 template <typename T, int K, int CB>
@@ -725,7 +718,7 @@ static int launch_gemm(const aqlm_b200_weight_t* w, const void* input, void* out
   {
     cuuint64_t dims[2] = {(cuuint64_t)w->in_features, (cuuint64_t)batch};
     cuuint64_t strides[1] = {(cuuint64_t)w->in_features * 2};
-    cuuint32_t box[2] = {(cuuint32_t)kGemmBlockK, (cuuint32_t)(g.n_tile / g.cluster)};
+    cuuint32_t box[2] = {(cuuint32_t)kGemmBlockK, (cuuint32_t)g.n_tile};
     cuuint32_t es[2] = {1, 1};
     CUresult r = enc(&tx, DT<T>::is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
                      const_cast<void*>(input), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -755,40 +748,15 @@ static int launch_gemm(const aqlm_b200_weight_t* w, const void* input, void* out
   p.nbits = w->nbits_per_codebook;
   p.total_kblocks = g.total_kblocks;
   p.ksplit = g.ksplit;
-  p.n_tile = g.n_tile;
   p.stages = g.stages;
-  p.a_stages = g.a_stages;
-  p.groups = g.groups;
   p.tile_m = g.tile_m;
-  p.cluster = g.cluster;
-  p.debug = tun().gemm_debug;
   p.gather_mode = tun().gemm_gather_mode >= 0 ? tun().gemm_gather_mode : (w->nbits_per_codebook > 8 ? 1 : 0);
-  p.codes = w->codes;
-  p.row_bytes = (long long)(w->in_features / 8) * K * CB;
-  const size_t smem = gemm_smem_layout(g.stages, g.n_tile, g.atmem).total;
-  const bool v2 = g.v2 && g.stages <= 4;
-  const bool atmem = g.atmem && v2;
-  auto kernel = atmem ? gemm_dequant_kernel<T, K, CB, true, true>
-                      : (v2 ? gemm_dequant_kernel<T, K, CB, true, false> : gemm_dequant_kernel<T, K, CB, false, false>);
-  static SmemMarks marks[3];
-  if (int rc = ensure_smem(kernel, smem, marks[atmem ? 2 : (v2 ? 1 : 0)], di)) return rc;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(g.m_tiles, g.ksplit, g.n_tiles);
-  cfg.blockDim = dim3(v2 ? kGemmThreadsV2 : kGemmThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = g.cluster;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = tun().pdl ? 1 : 0;
-  cfg.attrs = attr;
-  cfg.numAttrs = 2;
-  AQLM_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, tx, tc, p));
-  count_launch();
-  return AQLM_B200_OK;
+  switch (g.n_tile) {
+    case 16: return launch_gemm_n<T, K, CB, 16>(tx, tc, p, g, di, st);
+    case 32: return launch_gemm_n<T, K, CB, 32>(tx, tc, p, g, di, st);
+    case 64: return launch_gemm_n<T, K, CB, 64>(tx, tc, p, g, di, st);
+    default: return launch_gemm_n<T, K, CB, 128>(tx, tc, p, g, di, st);
+  }
 }
 
 template <typename T>
@@ -805,7 +773,7 @@ static int gemm_typed(const aqlm_b200_weight_t* w, const void* input, void* outp
   return launch_gemm<T, 8, 1>(w, input, output, batch, g, workspace, st);
 }
 
-// ---- fused dequant + TRANSPOSED tcgen05 GEMM (backward w.r.t. the input): host side ---------------------
+// ---- fused dequant + TRANSPOSED wgmma GEMM (backward w.r.t. the input): host side ---------------------
 struct GemmTPlan {
   bool ok = false;
   int m_tiles = 0, n_tiles = 0, n_tile = 0, ksplit = 1, stages = 0, total_kblocks = 0;
@@ -821,16 +789,10 @@ static GemmTPlan gemm_t_plan(const aqlm_b200_weight_t* w, int64_t batch, const D
   if (w->out_features % 8 != 0) return g;  // TMA row stride of grad_out
   if ((reinterpret_cast<uintptr_t>(w->codes) & 15) != 0) return g;
   if (((size_t)(w->in_features / 8) * K * cb) % 16 != 0) return g;
-  if (tun().disable_tcgen05) return g;
+  if (tun().disable_wgmma) return g;
   g.total_kblocks = (int)((w->out_features + kGemmBlockK - 1) / kGemmBlockK);
   g.m_tiles = (int)((w->in_features + kGemmBlockM - 1) / kGemmBlockM);
-  if (batch <= 256) {
-    g.n_tile = (int)((batch + 15) / 16 * 16);
-    g.n_tiles = 1;
-  } else {
-    g.n_tile = 256;
-    g.n_tiles = (int)((batch + 255) / 256);
-  }
+  gemm_n_tiles(batch, &g.n_tile, &g.n_tiles);
   const int ctile_row_bytes = 16 * K * cb;
   const size_t budget = (size_t)di->max_smem_optin;
   int S = 3;
@@ -841,12 +803,9 @@ static GemmTPlan gemm_t_plan(const aqlm_b200_weight_t* w, int64_t batch, const D
   if ((size_t)g.m_tiles * g.n_tiles > (size_t)kGemmMaxTiles) return g;
   int ks = 1;
   if (allow_split) {
-    // same cost model as the forward plan: a k-block costs max(gathers, tensor pipe, smem traffic), every wave pays a
-    // fixed ~5 us, split-K partials go through L2 once each way
-    const double clk = 1.9e9;
-    const double t_gather = 1024.0 * K / ((nbits == 16 ? 0.85 : 1.6) * 0.7);
-    const double t_smem = 256.0 + 2.0 * g.n_tile, t_mma = 2.0 * g.n_tile;
-    const double t_kb = (t_gather > t_smem ? (t_gather > t_mma ? t_gather : t_mma) : (t_smem > t_mma ? t_smem : t_mma)) + 60.0;
+    // same cost model as the forward plan; every wave pays a fixed ~5 us, split-K partials go through L2 once each way
+    const double clk = 1.7e9;
+    const double t_kb = gemm_kblock_clk(kGemmBlockM, K, nbits, g.n_tile, 2.0 * 128 * 128 + 3.0 * g.n_tile * 128);
     const double tiles = (double)g.m_tiles * g.n_tiles;
     double best = 1e30;
     const int max_ks = g.total_kblocks / 2 < 16 ? (g.total_kblocks / 2 < 1 ? 1 : g.total_kblocks / 2) : 16;
@@ -854,7 +813,7 @@ static GemmTPlan gemm_t_plan(const aqlm_b200_weight_t* w, int64_t batch, const D
       const double ctas = tiles * c;
       const double waves = (double)((long long)((ctas + di->sm_count - 1) / di->sm_count));
       const double kb_cta = (double)((g.total_kblocks + c - 1) / c);
-      const double fix = c > 1 ? ctas * g.n_tile * kGemmBlockM * 4.0 * 2.0 / 4e12 * clk : 0.0;
+      const double fix = c > 1 ? ctas * g.n_tile * kGemmBlockM * 4.0 * 2.0 / 3e12 * clk : 0.0;
       const double t = waves * (kb_cta * t_kb + 5e-6 * clk) + fix;
       if (t < best * 0.97) {
         best = t;
@@ -870,6 +829,28 @@ static GemmTPlan gemm_t_plan(const aqlm_b200_weight_t* w, int64_t batch, const D
   g.partials_bytes = ks > 1 ? (size_t)g.m_tiles * g.n_tiles * ks * g.n_tile * kGemmBlockM * 4 : 0;
   g.ok = true;
   return g;
+}
+
+template <typename T, int K, int CB, int N>
+static int launch_gemm_t_n(const CUtensorMap& tg, const CUtensorMap& tc, const GemmTParams& p, const GemmTPlan& g,
+                           const DeviceInfo* di, cudaStream_t st) {
+  const size_t smem = gemm_t_smem_layout(g.stages, N, 16 * K * CB).total;
+  auto kernel = gemm_dequant_t_kernel<T, K, CB, N>;
+  static SmemMarks marks;
+  if (int rc = ensure_smem(kernel, smem, marks, di)) return rc;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(g.m_tiles, g.ksplit, g.n_tiles);
+  cfg.blockDim = dim3(kGemmThreads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = tun().pdl ? 1 : 0;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  AQLM_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, tg, tc, p));
+  count_launch();
+  return AQLM_B200_OK;
 }
 
 template <typename T, int K, int CB>
@@ -915,26 +896,14 @@ static int launch_gemm_t(const aqlm_b200_weight_t* w, const void* grad_output, v
   p.nbits = w->nbits_per_codebook;
   p.total_kblocks = g.total_kblocks;
   p.ksplit = g.ksplit;
-  p.n_tile = g.n_tile;
   p.stages = g.stages;
   p.gather_mode = tun().gemm_gather_mode >= 0 ? tun().gemm_gather_mode : (w->nbits_per_codebook > 8 ? 1 : 0);
-  const size_t smem = gemm_t_smem_layout(g.stages, g.n_tile, GBT).total;
-  auto kernel = gemm_dequant_t_kernel<T, K, CB>;
-  static SmemMarks marks;
-  if (int rc = ensure_smem(kernel, smem, marks, di)) return rc;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(g.m_tiles, g.ksplit, g.n_tiles);
-  cfg.blockDim = dim3(kGemmTThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = tun().pdl ? 1 : 0;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  AQLM_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, tg, tc, p));
-  count_launch();
-  return AQLM_B200_OK;
+  switch (g.n_tile) {
+    case 16: return launch_gemm_t_n<T, K, CB, 16>(tg, tc, p, g, di, st);
+    case 32: return launch_gemm_t_n<T, K, CB, 32>(tg, tc, p, g, di, st);
+    case 64: return launch_gemm_t_n<T, K, CB, 64>(tg, tc, p, g, di, st);
+    default: return launch_gemm_t_n<T, K, CB, 128>(tg, tc, p, g, di, st);
+  }
 }
 
 template <typename T>
@@ -989,11 +958,11 @@ int aqlm_b200_matmat_ex(const aqlm_b200_weight_t* w, const void* input, void* ou
   if (batch == 0) return AQLM_B200_OK;
   if (!input || !output) return fail(AQLM_B200_ERR_SHAPE, "input/output pointer is NULL");
   const DeviceInfo* di = device_info();
-  if (!di) return (int)(strstr(tls_error_buf(), "sm_100a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
+  if (!di) return (int)(strstr(tls_error_buf(), "sm_90a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   {
     // batch 1 -- and batch 2-3 as one launch per row, like the reference's per-row host loop (cuda_kernel.cpp:387-421):
-    // measured faster than one pass of the gather kernel up to 3 rows (profiles/r02/probe_lut_*.jsonl)
+    // up to 3 rows this replaces one pass of the gather kernel (AQLM_B200_LUT_BATCH_LOOP=0 selects that pass instead)
     const int64_t lut_rows = (batch == 1 || (tun().lut_batch_loop && batch <= 3)) ? batch : 0;
     const size_t out_elt = partial ? 4 : 2;
     int64_t done = 0;
@@ -1027,7 +996,7 @@ int aqlm_b200_matmat_ws(const aqlm_b200_weight_t* w, const void* input, void* ou
   const int64_t ws_rows = (batch == 1 || (tun().lut_batch_loop && batch == 2 && w->num_codebooks >= 4)) ? batch : 0;
   if (ws_rows > 0 && workspace && input && output && (reinterpret_cast<uintptr_t>(input) & 3) == 0) {
     const DeviceInfo* di = device_info();
-    if (!di) return (int)(strstr(tls_error_buf(), "sm_100a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
+    if (!di) return (int)(strstr(tls_error_buf(), "sm_90a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (batch == 1) {  // K <= 2, in <= 4096: the cluster kernel needs no workspace (matmat_ex also loops it for batch 2-3)
       bool taken = false;
@@ -1068,7 +1037,7 @@ int aqlm_b200_matmat_grouped(const aqlm_b200_weight_t* w, const int64_t* seg_row
   if (row_bytes % 16 != 0 || (reinterpret_cast<uintptr_t>(w->codes) & 15) || (reinterpret_cast<uintptr_t>(input) & 15))
     return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped launch needs 16-byte aligned code rows and input");
   const DeviceInfo* di = device_info();
-  if (!di) return (int)(strstr(tls_error_buf(), "sm_100a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
+  if (!di) return (int)(strstr(tls_error_buf(), "sm_90a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
   GemvParams p;
   p.codes = w->codes;
   p.codebooks = w->codebooks;
@@ -1123,7 +1092,7 @@ int aqlm_b200_matmat_dequant_ws(const aqlm_b200_weight_t* w, const void* input, 
   if (batch == 0) return AQLM_B200_OK;
   if (!input || !output) return fail(AQLM_B200_ERR_SHAPE, "input/output pointer is NULL");
   const DeviceInfo* di = device_info();
-  if (!di) return (int)(strstr(tls_error_buf(), "sm_100a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
+  if (!di) return (int)(strstr(tls_error_buf(), "sm_90a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   GemmPlan g = gemm_plan(w, batch, di, workspace != nullptr);
   if (g.ok && g.ksplit > 1 && workspace_bytes < g.counters_bytes + g.partials_bytes) g = gemm_plan(w, batch, di, false);
@@ -1146,7 +1115,7 @@ int aqlm_b200_dequant(const aqlm_b200_weight_t* w, void* weight_out, int apply_s
   if (rc) return rc;
   if (!weight_out || (reinterpret_cast<uintptr_t>(weight_out) & 15))
     return fail(AQLM_B200_ERR_SHAPE, "weight_out must be a 16-byte aligned device pointer");
-  if (!device_info()) return (int)(strstr(tls_error_buf(), "sm_100a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
+  if (!device_info()) return (int)(strstr(tls_error_buf(), "sm_90a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (w->dtype == AQLM_B200_F16) return dequant_typed<__half>(w, weight_out, apply_scales, st);
   return dequant_typed<__nv_bfloat16>(w, weight_out, apply_scales, st);
@@ -1171,7 +1140,7 @@ int aqlm_b200_matmat_dequant_transposed(const aqlm_b200_weight_t* w, const void*
   if ((reinterpret_cast<uintptr_t>(grad_output) & 15) != 0)
     return fail(AQLM_B200_ERR_SHAPE, "grad_output must be 16-byte aligned");
   const DeviceInfo* di = device_info();
-  if (!di) return (int)(strstr(tls_error_buf(), "sm_100a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
+  if (!di) return (int)(strstr(tls_error_buf(), "sm_90a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
   GemmTPlan g = gemm_t_plan(w, batch, di, workspace != nullptr);
   if (g.ok && g.ksplit > 1 && workspace_bytes < g.counters_bytes + g.partials_bytes) g = gemm_t_plan(w, batch, di, false);
   if (!g.ok)
@@ -1188,7 +1157,7 @@ int aqlm_b200_scale_bias(const float* partial, const void* scales, const void* b
   if (!partial || !scales || !output) return fail(AQLM_B200_ERR_SHAPE, "NULL pointer");
   if (dtype != AQLM_B200_F16 && dtype != AQLM_B200_BF16) return fail(AQLM_B200_ERR_DTYPE, "dtype must be f16/bf16");
   if (batch <= 0 || out_features <= 0) return AQLM_B200_OK;
-  if (!device_info()) return (int)(strstr(tls_error_buf(), "sm_100a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
+  if (!device_info()) return (int)(strstr(tls_error_buf(), "sm_90a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int64_t n = batch * out_features;
   const unsigned blocks = (unsigned)((n + 255) / 256);
@@ -1274,7 +1243,7 @@ int aqlm_b200_allreduce_scale_bias(aqlm_b200_comm* c, const float* partial, cons
   if (n <= 0) return AQLM_B200_OK;
   if (n > c->max_elems || (out_features & 3)) return fail(AQLM_B200_ERR_SHAPE, "allreduce: %lld elements exceed the communicator's %lld (or out_features %% 4 != 0)", (long long)n, c->max_elems);
   const DeviceInfo* di = device_info();
-  if (!di) return (int)(strstr(tls_error_buf(), "sm_100a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
+  if (!di) return (int)(strstr(tls_error_buf(), "sm_90a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
   PeerParams p;
   for (int r = 0; r < kPeerMaxWorld; ++r) p.peer_base[r] = r < c->world ? c->peer_base[r] : nullptr;
   p.local = partial;
@@ -1323,7 +1292,7 @@ int aqlm_b200_matmat_allreduce(aqlm_b200_comm* c, const aqlm_b200_weight_t* w, c
   if (row_bytes % 16 != 0 || (reinterpret_cast<uintptr_t>(w->codes) & 15) || (reinterpret_cast<uintptr_t>(input) & 15))
     return fail(AQLM_B200_ERR_UNSUPPORTED, "fused exchange needs 16-byte aligned code rows and input");
   const DeviceInfo* di = device_info();
-  if (!di) return (int)(strstr(tls_error_buf(), "sm_100a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
+  if (!di) return (int)(strstr(tls_error_buf(), "sm_90a") ? AQLM_B200_ERR_ARCH : AQLM_B200_ERR_CUDA);
   GemvParams p;
   p.codes = w->codes;
   p.codebooks = w->codebooks;

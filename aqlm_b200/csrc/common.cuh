@@ -1,4 +1,4 @@
-// Common device/host helpers for the aqlm_b200 kernels (sm_100a only).
+// Common device/host helpers for the aqlm_b200 kernels (sm_90a only).
 #pragma once
 
 #include <cuda_bf16.h>
@@ -112,19 +112,12 @@ __device__ __forceinline__ uint4 ld_gather_v4(const void* p) {
   return r;
 }
 
-// 32-byte gather (in_group_size = 16: one codebook entry = one 32-byte L2 sector) as ONE 256-bit request (LDG.E.256,
-// sm_100+) instead of two 128-bit requests to the same sector: the gather kernels are bound by requests, not bytes.
+// 32-byte gather (in_group_size = 16: one codebook entry = one 32-byte L2 sector).  sm_90 has no 256-bit load, so
+// the entry is read as two 128-bit requests to the same sector, issued back to back.
 template <int MODE>
 __device__ __forceinline__ void ld_gather_v8(const void* p, uint4& lo, uint4& hi) {
-  if constexpr (MODE == 1) {
-    asm volatile("ld.global.cg.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(lo.x), "=r"(lo.y), "=r"(lo.z), "=r"(lo.w), "=r"(hi.x), "=r"(hi.y), "=r"(hi.z), "=r"(hi.w)
-                 : "l"(p));
-  } else {
-    asm volatile("ld.global.nc.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(lo.x), "=r"(lo.y), "=r"(lo.z), "=r"(lo.w), "=r"(hi.x), "=r"(hi.y), "=r"(hi.z), "=r"(hi.w)
-                 : "l"(p));
-  }
+  lo = ld_gather_v4<MODE == 1 ? 1 : 0>(p);
+  hi = ld_gather_v4<MODE == 1 ? 1 : 0>(reinterpret_cast<const uint4*>(p) + 1);
 }
 
 // Programmatic dependent launch (PDL).  Both are no-ops when the kernel was launched without the

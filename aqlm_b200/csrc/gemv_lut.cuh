@@ -214,8 +214,7 @@ __global__ void __launch_bounds__(kLutThreads, (kLutThreads == 256) ? 2 : 1) gem
   // The grid is one resident wave (host side guarantees it), so the n_slabs CTAs of a row block can rendezvous: each
   // publishes its partials, takes a ticket, and the last arrival bumps the block's generation word; everybody then adds
   // the slabs IN SLAB ORDER (deterministic) for its own 1/n_slabs share of the rows (32-row chunks dealt round-robin).
-  // Before: only the last-arriving CTA did the whole block (n_slabs x rows loads behind one L2 round trip each) --
-  // measured 4.8 us of an 11.8 us kernel at 4096->11008 2x8 and 8.8 of 16.5 us at 11008->4096 (profiles/r02/probe_lut.jsonl).
+  // (Letting only the last-arriving CTA do the whole block puts n_slabs x rows loads behind one L2 round trip each.)
   unsigned int* s_gen = reinterpret_cast<unsigned int*>(lut + (size_t)K * 256 * J);
   if (tid == 0) *s_gen = *reinterpret_cast<volatile unsigned int*>(p.ws_gen + rb);  // cannot advance before I arrive
   __threadfence();
@@ -264,7 +263,7 @@ __global__ void __launch_bounds__(kLutThreads, (kLutThreads == 256) ? 2 : 1) gem
 // ---------------------------------------------------------------------------------------------------
 // Cluster variant for K = 1, 2 and in_features <= 8 slabs of 64 groups (4096 for g = 8): the slab CTAs of a row block form
 // ONE thread-block cluster and reduce their partial rows through DISTRIBUTED SHARED MEMORY -- no global partials, no
-// fence/atomic/poll round trips (those cost 3.8 us of an 11 us kernel, profiles/r02/probe_lut_c.jsonl).
+// fence/atomic/poll round trips through global memory.
 //   * slab = 64 in-groups, LUT [K][256][64] fp32 (64/128 KiB), 512 threads, one CTA per SM;
 //   * a lane owns the ADJACENT groups 2l, 2l+1: one aligned code word per row (K=2: 4 bytes, K=1: 2 bytes) = a fully
 //     coalesced 128/64-byte row segment per warp; group 2l sits at LUT position l, group 2l+1 at position 32+l, so both
@@ -458,8 +457,8 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_lut_cluster_kernel(const LutC
 
 // ---------------------------------------------------------------------------------------------------
 // Cluster kernel, second form (default for K <= 2, in_features <= 8 slabs of 64 groups).  Same slab / lane <-> adjacent-group
-// layout and the same tensor-core LUT build as gemv_lut_cluster_kernel; three changes, each aimed at a measured cost
-// (profiles/r02/probe_lut_d.jsonl: lookups 2.9 us, cross-slab sum 1.6 us of an 8.9 us kernel at 2x8 4096->11008):
+// layout and the same tensor-core LUT build as gemv_lut_cluster_kernel; three changes, aimed at the cost of the lookups
+// and of the cross-slab sum:
 //   * ONE instruction of address arithmetic per lookup.  The LUT is placed at the first 64 KiB boundary of the CTA's
 //     shared window above the receive buffers (window offset 0x10000; codebook k at 0x10000 * (1 + k)); a LUT row (one entry, 64 groups) is 256 bytes, so the address of entry `code` for
 //     the lane's group is  {byte3, byte2, byte1, byte0} = {base.hi, base.lo + k, code, 4 * lane}  -- one PRMT that takes the code byte

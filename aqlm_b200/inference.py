@@ -1,4 +1,4 @@
-"""`QuantizedLinear`: the module-level API of the AQLM hot path, CUDA (sm_100a) only.
+"""`QuantizedLinear`: the module-level API of the AQLM hot path, CUDA (sm_90a) only.
 
 Public contract kept from the reference module (inference_lib/src/aqlm/inference.py:11-142), because Hugging Face's AQLM
 integration and existing checkpoints depend on it:
@@ -85,7 +85,7 @@ class QuantizedLinear(nn.Module):
         """Bind the four ops for this module's scheme (reference inference.py:77-96).  CUDA only."""
         if not input.is_cuda:
             raise NotImplementedError(
-                f"aqlm_b200.QuantizedLinear runs on CUDA (sm_100a) only; got input on {input.device}. "
+                f"aqlm_b200.QuantizedLinear runs on CUDA (sm_90a) only; got input on {input.device}. "
                 "There is no CPU fallback in this package.")
         self._ops = tuple(select(self.codebooks, large_batch)
                           for large_batch in (False, True)

@@ -5,7 +5,7 @@ Mirrors what the reference registers (cuda_kernel.py:13-132): torch.library ops
 `(Tensor input, Tensor codes, Tensor codebooks, Tensor scales, Tensor? bias) -> Tensor` plus fake/meta shapes so
 `torch.compile` / CUDA-graph capture work, and a `CUDA_KERNEL` namespace exposing the functions the reference's
 pybind module exports (cuda_kernel.cpp:686-699; used by benchmark/matmul_benchmark.py:103).  Differences:
-no JIT build at import (the .so is prebuilt in-tree for sm_100a), `aqlm::generic_matmat[_dequant]` covers every
+no JIT build at import (the .so is prebuilt in-tree for sm_90a), `aqlm::generic_matmat[_dequant]` covers every
 other KxN scheme (the reference sends those to Triton, kernel_selector.py:91-94), and CPU tensors are an error.
 """
 from __future__ import annotations
@@ -41,7 +41,7 @@ def _require_cuda(*tensors: Optional[torch.Tensor]) -> torch.device:
             continue
         if not t.is_cuda:
             raise NotImplementedError(
-                "aqlm_b200 implements the CUDA (sm_100a) hot path only; got a tensor on "
+                "aqlm_b200 implements the CUDA (sm_90a) hot path only; got a tensor on "
                 f"{t.device}. There is no CPU fallback in this package.")
         if dev is None:
             dev = t.device
@@ -170,7 +170,7 @@ def matmat(input, codes, codebooks, scales, bias=None) -> torch.Tensor:
 
 
 def matmat_dequant(input, codes, codebooks, scales, bias=None) -> torch.Tensor:
-    """Fused dequant + tcgen05 tensor-core GEMM (+scale+bias); for large batch (reference `*_matmat_dequant`)."""
+    """Fused dequant + wgmma tensor-core GEMM (+scale+bias); for large batch (reference `*_matmat_dequant`)."""
     device, w, flat_input = _prepare(input, codes, codebooks, scales, bias)
     batch = flat_input.shape[0]
     flat_output = torch.empty((batch, w.out_features), dtype=input.dtype, device=device)
@@ -248,7 +248,7 @@ def dequant(codes, codebooks, scales=None) -> torch.Tensor:
 def matmat_dequant_transposed(input, codes, codebooks, scales, bias=None) -> torch.Tensor:
     """Backward w.r.t. the input: grad_in = (grad_out * scales) @ W_unscaled (reference cuda_kernel.cpp:303-354).
 
-    ONE fused kernel (csrc/gemm_tcgen05_t.cuh): W^T tiles are dequantized on chip into an MN-major tcgen05 operand, the
+    ONE fused kernel (csrc/gemm_wgmma_t.cuh): W^T tiles are dequantized on chip into an MN-major wgmma operand, the
     per-row scale is folded into the tile, grad_out tiles arrive by TMA; W is never materialised and no library GEMM is
     called.  The reference's 2x8/1x8 variants forget the scaled input (cuda_kernel.cpp:497,518,662,683); not reproduced.
     `bias` is the forward bias [out]; it has no place in grad_input (the reference passes it to F::linear,
@@ -300,7 +300,7 @@ def _fake_transposed(input, codes, codebooks, scales, bias=None):
 
 
 def _cpu_refusal(*args, **kwargs):
-    raise NotImplementedError("aqlm_b200 ops run on CUDA (sm_100a) only; there is no CPU fallback in this package")
+    raise NotImplementedError("aqlm_b200 ops run on CUDA (sm_90a) only; there is no CPU fallback in this package")
 
 
 def _register(name: str, fn, fake) -> None:

@@ -27,7 +27,7 @@ def _scheme_prefix(codebooks: torch.Tensor) -> str:
     num_codebooks, codebook_size, out_group_size, in_group_size = codebooks.shape
     if codebooks.device.type != "cuda":
         raise NotImplementedError(
-            f"aqlm_b200 implements the CUDA (sm_100a) hot path only; codebooks are on {codebooks.device}. "
+            f"aqlm_b200 implements the CUDA (sm_90a) hot path only; codebooks are on {codebooks.device}. "
             "Use the reference `aqlm` package for CPU inference.")
     if out_group_size != 1:
         raise NotImplementedError(f"aqlm_b200 kernels require out_group_size == 1, got {out_group_size}")

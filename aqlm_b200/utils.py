@@ -49,7 +49,7 @@ def _dequantize_weight(codes: torch.Tensor, codebooks: torch.Tensor,
 
     if not codebooks.is_cuda:
         raise NotImplementedError(
-            "aqlm_b200._dequantize_weight runs on CUDA (sm_100a) only; there is no CPU fallback in this package")
+            "aqlm_b200._dequantize_weight runs on CUDA (sm_90a) only; there is no CPU fallback in this package")
     nbits = codebooks.shape[1].bit_length() - 1
     storage = get_int_dtype(nbits)
     if codes.dtype != storage:

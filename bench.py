@@ -1,19 +1,22 @@
 #!/usr/bin/env python
-"""bench.py -- AQLM quantized-linear hot path on B200: matvec GB/s (code bytes) & tok/s vs the HBM roofline.
+"""bench.py -- AQLM quantized-linear hot path on H100: matvec GB/s (code bytes) & tok/s vs the HBM roofline.
 
-Contract (see DESIGN.md §Measurement):
+Usage:
   python bench.py --gpus N --steps K --warmup W        one JSON line on stdout (rank 0)
-  python bench.py --impl reference ...                 the reference's OWN CPU code (baseline/_ref, unmodified) on host cores
+  python bench.py --impl reference ...                 the reference's OWN CPU code (oracle/_ref, unmodified) on host cores
 
 A "step" is ONE decode-token pass over every quantized linear of the model named in `config.workload`
 (q,k,v,o,gate,up,down x n_layers; batch 1; linears only), each linear with its own codes/codebooks/scales so a step
-streams the whole model's codes from HBM (1.6 GiB for Llama-3-8B >> 126 MB L2: inputs larger than L2, no flush needed).
+streams the whole model's codes from HBM (1.6 GiB for Llama-3-8B >> 50 MB L2: inputs larger than L2, no flush needed).
   N == 1 : workload = BASELINE.json configs[1], Llama-3-8B 1x16 g8 (override with --workload/--scheme)
   N  > 1 : workload = BASELINE.json configs[4], Llama-3-70B 1x16, every linear sharded along in_features across the N
            ranks, fp32 partials, ONE NCCL all-reduce per linear, scale+bias after the reduce ("strong" scaling).
 `value`   = code bytes of the whole model / step time, inputs resident in HBM, step replayed as one CUDA graph.
 `e2e`     = same metric through the public module API with the activations coming from pinned HOST memory every
             step (H2D) and the last linear's output read back (D2H), both inside the timed region.
+--dump-outputs DIR writes what the last timed step computed: per linear, the outputs of every layer as
+DIR/<linear>.npy (float32, [layers, batch, out_features]).  Weights and activations come from fixed seeds, so two builds
+run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -59,7 +62,7 @@ def measured_peaks():
             p = json.load(f)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 class Watchdog:
@@ -94,7 +97,7 @@ class Watchdog:
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -189,11 +192,11 @@ def cpu_layer_sample(model, K, nbits, target_seconds, nthreads=0):
                        f"{reps} reps, {kernel}", tok_s=1.0 / (dt * MODELS[model]["layers"]))
 
 
-REF_DIR = os.path.join(REPO, "baseline", "_ref")
+REF_DIR = os.path.join(REPO, "oracle", "_ref")
 
 
 def import_reference_aqlm():
-    """The UNMODIFIED reference package, pip-installed into the git-ignored baseline/_ref (it travels to the GPU box).
+    """The UNMODIFIED reference package, pip-installed into the git-ignored oracle/_ref (it travels to the GPU box).
     Only its CPU path is used here (QuantizedLinear.forward -> dequantize_gemm / numba_gemm_lut); its CUDA extension is
     never imported in this process."""
     if not os.path.isdir(os.path.join(REF_DIR, "aqlm")):
@@ -237,7 +240,7 @@ def cpu_reference_layer_sample(model, K, nbits, target_seconds, numba_threads=1)
     layer's 7 linears, bs=1, fp32 (the dtype of benchmark/matmul_benchmark_cpu.py:114-123).  1x16 resolves to
     `dequantize_gemm` (kernel_selector.py:99-102; torch intra-op threads = all cores); 256-entry codebooks resolve to the
     Numba LUT kernel (kernel_selector.py:95-98, numba_kernel.py:10-65) with NUMBA_NUM_THREADS=1, the reference benchmark's
-    default (`--nthreads 1`) and the only race-free setting.  Returns None when baseline/_ref is absent."""
+    default (`--nthreads 1`) and the only race-free setting.  Returns None when oracle/_ref is absent."""
     lut = 2**nbits == 256
     if lut:
         os.environ.setdefault("NUMBA_NUM_THREADS", str(numba_threads))
@@ -278,8 +281,8 @@ def cpu_reference_layer_sample(model, K, nbits, target_seconds, numba_threads=1)
         one_pass()
     dt = (time.perf_counter() - t0) / reps
     cores = numba_threads if lut else torch.get_num_threads()
-    kernel = ("aqlm.inference_kernels.numba_kernel.numba_gemm_lut (baseline/_ref, NUMBA_NUM_THREADS=%d)" % numba_threads) if lut \
-        else "aqlm.inference_kernels.dequantization.dequantize_gemm (baseline/_ref, torch CPU ops)"
+    kernel = ("aqlm.inference_kernels.numba_kernel.numba_gemm_lut (oracle/_ref, NUMBA_NUM_THREADS=%d)" % numba_threads) if lut \
+        else "aqlm.inference_kernels.dequantization.dequantize_gemm (oracle/_ref, torch CPU ops)"
     return dict(value=nbytes / dt / 1e9, unit="GB/s", cores=cores, kind="reference", seconds_per_layer=dt,
                 sample=f"one decoder layer (7 linears, {nbytes / 2**20:.1f} MiB of codes) of {model} {K}x{nbits}, bs=1, fp32, "
                        f"{reps} reps through the reference's own QuantizedLinear.forward on CPU: {kernel}",
@@ -287,7 +290,7 @@ def cpu_reference_layer_sample(model, K, nbits, target_seconds, numba_threads=1)
 
 
 def cpu_baseline_sample(model, K, nbits, target_seconds):
-    """cpu_baseline object: the reference's own CPU code when baseline/_ref is present (kind "reference"), with the
+    """cpu_baseline object: the reference's own CPU code when oracle/_ref is present (kind "reference"), with the
     oracle's C port (all cores) reported beside it; the port alone (kind "port") otherwise."""
     ref = cpu_reference_layer_sample(model, K, nbits, target_seconds)
     port = cpu_layer_sample(model, K, nbits, target_seconds=min(target_seconds, 8.0))
@@ -298,9 +301,9 @@ def cpu_baseline_sample(model, K, nbits, target_seconds):
 
 
 def run_reference(args):
-    """`--impl reference`: the reference's own CPU implementation of the path -- the UNMODIFIED package in baseline/_ref,
+    """`--impl reference`: the reference's own CPU implementation of the path -- the UNMODIFIED package in oracle/_ref,
     through its public module API (`aqlm.QuantizedLinear.forward` on CPU tensors) -- on the box's host cores; a bounded
-    sample per step = one decoder layer.  Falls back to the oracle port only when baseline/_ref is not installed."""
+    sample per step = one decoder layer.  Falls back to the oracle port only when oracle/_ref is not installed."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
@@ -489,7 +492,7 @@ def _tool(argv, timeout):
 
 
 def secondary_metrics(device, peak_hbm, args):
-    """Extra measurements reported beside the headline (not part of `value`): the fused dequant + tcgen05 GEMM (BASELINE
+    """Extra measurements reported beside the headline (not part of `value`): the fused dequant + wgmma GEMM (BASELINE
     configs[3]), the Kx8 matvec on every Llama-2-7B shape (configs[2]), the other schemes of SURVEY §8 f4 (1x8, 1x16 g=16,
     bf16), the reference's own CUDA kernels and Numba CPU kernel timed in the same job, and HF `generate` tok/s (§8 f1).
     Matvec/GEMM numbers: CUDA-graph replay over rotating weight copies (codes come from HBM), CUDA events."""
@@ -501,7 +504,7 @@ def secondary_metrics(device, peak_hbm, args):
         with open(os.path.join(REPO, "MEASURED_PEAKS.json")) as f:
             tpeak = float(json.load(f)["bf16_tflops"])
     except Exception:
-        tpeak = 1590.0
+        tpeak = 989.0  # H100 SXM data sheet, dense BF16
 
     def timed(fns, iters=10):
         for f in fns:
@@ -582,7 +585,7 @@ def secondary_metrics(device, peak_hbm, args):
     out["tensor_peak_tflops"] = tpeak
     torch.cuda.empty_cache()
     if not args.skip_reference_gpu and os.path.isdir(os.path.join(REF_DIR, "aqlm")):
-        # the reference's stock CUDA kernels (baseline/_ref, JIT-built for sm_100) with the same timing protocol
+        # the reference's stock CUDA kernels (oracle/_ref, JIT-built for sm_90) with the same timing protocol
         out["reference_gpu"] = _tool([os.path.join("tools", "compare_reference_gpu.py"), "--cases", "quick"], timeout=420)
         out["generate"] = {
             "ours_fused": _tool([os.path.join("tools", "generate_benchmark.py"), "--impl", "ours", "--fuse", "--output_length", "64",
@@ -601,6 +604,20 @@ def secondary_metrics(device, peak_hbm, args):
         except Exception as e:
             out["reference_cpu_numba_2x8"] = {"error": f"{type(e).__name__}: {e}"}
     return out
+
+
+def dump_outputs(out_dir, model, ys, n_layers):
+    """Write the outputs of one step, grouped by linear: DIR/<linear>.npy = float32 [layers, batch, out_features].  The step
+    yields each layer's linears in layer_linears() order (a grouped launch yields its members in that order too)."""
+    import numpy as np
+
+    names = [name for name, _, _ in layer_linears(model)]
+    if len(ys) != n_layers * len(names):
+        raise RuntimeError(f"--dump-outputs: {len(ys)} outputs for {n_layers} layers x {len(names)} linears")
+    os.makedirs(out_dir, exist_ok=True)
+    for j, name in enumerate(names):
+        arr = np.stack([ys[i * len(names) + j].float().cpu().numpy() for i in range(n_layers)])
+        np.save(os.path.join(out_dir, f"{name}.npy"), arr)
 
 
 def run_ours(args):
@@ -656,16 +673,19 @@ def run_ours(args):
     if grouped:
         layers = group_layers(layers, K, nbits, world)
     in_sizes = sorted({n for mods in layers for _, n in mods})
-    x_dev = {n: torch.randn((1, n), dtype=torch.float16, device=device) for n in in_sizes}
-    x_host = {n: torch.randn((1, n), dtype=torch.float16).pin_memory() for n in in_sizes}
+    xgen = torch.Generator().manual_seed(4242)  # the same activations in every run (--dump-outputs compares builds)
+    x_host = {n: torch.randn((1, n), dtype=torch.float16, generator=xgen).pin_memory() for n in in_sizes}
+    x_dev = {n: x_host[n].to(device) for n in in_sizes}
     outs = {}
 
     def step():
-        y = None
+        y, ys = None, []
         for mods in layers:
             for m, n in mods:
                 y = m(x_dev[n])
+                ys.extend(y if isinstance(y, tuple) else (y,))
         outs["y"] = y[-1] if isinstance(y, tuple) else y
+        outs["all"] = ys
 
     # bind kernels / NCCL outside capture, count launches of one step
     step()
@@ -713,6 +733,8 @@ def run_ours(args):
     sampler = ClockSampler(local_rank) if rank == 0 else None
     ms_total = timed(run, args.steps)
     ms_step = ms_total / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, outs["all"], n_layers)
 
     # ---- e2e: pinned-host activations in, last output out, every step ---------------------------------
     y_host = torch.empty_like(outs["y"], device="cpu").pin_memory()
@@ -892,15 +914,6 @@ def run_ours(args):
             cpu = {k: cpu_full[k] for k in ("value", "unit", "cores", "kind", "sample")}
             if "port" in cpu_full:
                 cpu["port"] = cpu_full["port"]
-        traffic = None
-        tpath = os.path.join(REPO, "profiles", "ncu_traffic.json")
-        if os.path.exists(tpath):
-            try:
-                with open(tpath) as f:
-                    key = f"{model}:{K}x{nbits}:bytes_per_launch" if world == 1 else f"{model}:{K}x{nbits}:n{world}:bytes_per_launch"
-                    traffic = json.load(f).get(key)
-            except Exception:
-                traffic = None
         line = {
             "metric": "aqlm_matvec_code_GBps", "value": value, "unit": "GB/s", "n_gpus": world, "steps": args.steps,
             "warmup": max(3, args.warmup), "ms_per_step": ms_step, "higher_is_better": True,
@@ -913,7 +926,7 @@ def run_ours(args):
                        "grouped_launches": "q/k/v and gate/up each run as ONE grouped launch (QuantizedLinearGroup): 4 launches per layer"
                        if grouped else "one launch per linear (7 per layer)"},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "peak_source": peak_src,
+                         "peak_source": peak_src,
                          "kernel": "gemv (fused code-gather + dequant + dot), avg over the step's launches incl. launch gaps",
                          "avg_launch_us": avg_launch_us, "algorithmic_bytes_per_launch": per_gpu_bytes / n_lin},
             "e2e": {"value": e2e_value, "unit": "GB/s", "ms_per_step": ms_e2e, "tok_s_linears_only": 1e3 / ms_e2e,
@@ -972,7 +985,7 @@ def run_ours(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=100)
+    ap.add_argument("--steps", type=int, default=100, help="timed steps")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default=None, choices=[None, *MODELS])
@@ -988,7 +1001,11 @@ def main():
     ap.add_argument("--skip-reference-gpu", action="store_true", help="skip the reference CUDA kernels / generate legs")
     ap.add_argument("--watchdog-seconds", type=float, default=420.0,
                     help="N>1: leave with an error line if one phase (parity, build, timing, ...) takes longer than this (0: off)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<linear>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     if args.impl == "reference":
         run_reference(args)
     else:

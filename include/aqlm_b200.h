@@ -1,5 +1,5 @@
 /*
- * aqlm_b200 -- C-ABI of the B200-native (sm_100a) AQLM quantized-linear hot path.
+ * aqlm_b200 -- C-ABI of the H100-native (sm_90a) AQLM quantized-linear hot path.
  *
  * This header is the drop-in boundary (SURVEY.md §8b).  Every entry point takes plain device (or,
  * for *_host, pinned host) pointers, sizes and a CUstream/cudaStream_t passed as `void*`; no torch types.
@@ -36,7 +36,7 @@ typedef enum {
   AQLM_B200_ERR_UNSUPPORTED = 2, /* scheme/group size not implemented -> NotImplementedError (cuda_kernel.cpp:137-144) */
   AQLM_B200_ERR_SHAPE = 3,       /* inconsistent sizes / misaligned pointers -> ValueError */
   AQLM_B200_ERR_CUDA = 4,        /* CUDA runtime error (the reference never checks; we do) -> RuntimeError */
-  AQLM_B200_ERR_ARCH = 5         /* device is not sm_100 -> RuntimeError */
+  AQLM_B200_ERR_ARCH = 5         /* device is not sm_90 -> RuntimeError */
 } aqlm_b200_status;
 
 typedef enum { AQLM_B200_F16 = 0, AQLM_B200_BF16 = 1 } aqlm_b200_dtype;
@@ -110,7 +110,7 @@ int aqlm_b200_matmat_dequant_ws(const aqlm_b200_weight_t* w, const void* input, 
 int aqlm_b200_dequant(const aqlm_b200_weight_t* w, void* weight_out, int apply_scales, void* stream);
 
 /* Backward w.r.t. the input, fused: grad_input[batch, in] = (grad_output[batch, out] * scales) @ W_unscaled, with W
- * dequantized on chip (MN-major A tile, tcgen05 MMA, scale folded into the tile) -- W never goes to HBM and no library
+ * dequantized on chip (MN-major A tile, wgmma, scale folded into the tile) -- W never goes to HBM and no library
  * GEMM is involved.  Replaces code*_matmat_dequant_transposed (cuda_kernel.cpp:303-354, 486-519, 651-684: Dequant
  * kernel -> full W in HBM -> cuBLAS), with the 2x8/1x8 unscaled-input defect (cuda_kernel.cpp:497,518,662,683) NOT
  * reproduced.  The optional workspace (same zero-init contract as aqlm_b200_matmat_dequant_ws) enables split-K over the

@@ -1,7 +1,7 @@
 """Checkpoint-format path (SURVEY §8 f2): a synthetic Llama checkpoint written in the reference converter's format
 (convert_to_hf.py:50-100: config.json `quantization_config` block, `<linear>.codes` packed ints, `.codebooks`/`.scales`
 fp16, everything else fp16) must load through `AutoModelForCausalLM.from_pretrained` -- Hugging Face's own AQLM
-integration -- into OUR `QuantizedLinear` modules, report a version through `importlib.metadata`, and on a B200 produce
+integration -- into OUR `QuantizedLinear` modules, report a version through `importlib.metadata`, and on an H100 produce
 the logits of a dense model holding the dequantized weights.
 
 Environment notes: (1) the image has no `accelerate`; HF's AQLM quantizer only CHECKS for it (`validate_environment`),

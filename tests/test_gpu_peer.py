@@ -104,7 +104,7 @@ def test_one_process_two_devices_opt_in_shared_memory():
     from aqlm_b200.inference_kernels import cuda_kernel
 
     for dev in ("cuda:0", "cuda:1"):
-        for K, nbits, batch in ((2, 8, 1), (1, 16, 64), (1, 16, 5)):  # LUT GEMV, tcgen05 GEMM, batched gather GEMV
+        for K, nbits, batch in ((2, 8, 1), (1, 16, 64), (1, 16, 5)):  # LUT GEMV, wgmma GEMM, batched gather GEMV
             t = gpu_case(4096, 4096, K, nbits, batch, seed=K + batch, device=dev)
             op = cuda_kernel.matmat_dequant if batch > 6 else cuda_kernel.matmat
             y = op(t["x"], t["codes"], t["codebooks"], t["scales"], None)

@@ -1,8 +1,8 @@
-"""Time the UNMODIFIED reference CUDA kernels (pip-installed into the git-ignored baseline/_ref) on this GPU with the
+"""Time the UNMODIFIED reference CUDA kernels (pip-installed into the git-ignored oracle/_ref) on this GPU with the
 same protocol as tools/probe_gemv.py (CUDA-graph replay over rotating weight copies, CUDA events).
 
 Run in its OWN process (the reference and aqlm_b200 both register `aqlm::` torch.library ops):
-    TORCH_CUDA_ARCH_LIST=10.0 python tools/compare_reference_gpu.py [--out FILE]
+    TORCH_CUDA_ARCH_LIST=9.0 python tools/compare_reference_gpu.py [--out FILE]
 The reference JIT-builds its extension on first import (cuda_kernel.py:8-11); ~1 minute.
 """
 import argparse
@@ -11,12 +11,12 @@ import os
 import sys
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(REPO, "baseline", "_ref"))
-os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+sys.path.insert(0, os.path.join(REPO, "oracle", "_ref"))
+os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0")
 
 import torch  # noqa: E402
 
-L2_BYTES = 126 * 2**20
+L2_BYTES = 50 * 2**20  # H100 SXM
 
 
 def time_graph(fn_list, iters=20):
@@ -45,7 +45,7 @@ def main():
     ap.add_argument("--cases", default="all", choices=["all", "quick"], help="quick: the subset bench.py reports in `secondary`")
     args = ap.parse_args()
     import aqlm  # the reference
-    assert "baseline/_ref" in aqlm.__file__, aqlm.__file__
+    assert "oracle/_ref" in aqlm.__file__, aqlm.__file__
     from aqlm.inference_kernels.cuda_kernel import CUDA_KERNEL  # JIT build
 
     dev = "cuda:0"
@@ -89,7 +89,7 @@ def main():
             torch.cuda.synchronize()
             us = a.elapsed_time(b) * 1e3 / len(ws)
             mode = f"eager ({type(e).__name__})"
-        row = dict(impl="reference (baseline/_ref, unmodified, JIT sm_100)", op=name, scheme=scheme, in_features=fin,
+        row = dict(impl="reference (oracle/_ref, unmodified, JIT sm_90)", op=name, scheme=scheme, in_features=fin,
                    out_features=fout, batch=bs, us=round(us, 2), code_GBps=round(cbytes / us / 1e3, 1),
                    tflops=round(2.0 * bs * fin * fout / us / 1e6, 1), timing=mode)
         rows.append(row)

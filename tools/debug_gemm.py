@@ -1,4 +1,4 @@
-"""Diagnose tcgen05 GEMM mismatches: per-M-tile / per-column error map, repeated runs, env overrides."""
+"""Diagnose wgmma GEMM mismatches: per-M-tile / per-column error map, repeated runs, env overrides."""
 import os
 import sys
 
@@ -38,7 +38,7 @@ def run(fin, fout, batch, reps=3, label=""):
 
 if __name__ == "__main__":
     for env in ({}, {"AQLM_B200_GEMM_KSPLIT": "1"}, {"AQLM_B200_GEMM_KSPLIT": "2"}, {"AQLM_B200_GEMM_KSPLIT": "5"}):
-        for k in ("AQLM_B200_GEMM_STAGES", "AQLM_B200_GEMM_KSPLIT", "AQLM_B200_GEMM_DEBUG"):
+        for k in ("AQLM_B200_GEMM_STAGES", "AQLM_B200_GEMM_KSPLIT"):
             os.environ.pop(k, None)
         os.environ.update(env)
         from aqlm_b200 import _cabi

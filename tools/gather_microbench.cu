@@ -1,11 +1,11 @@
-// Microbenchmark: how fast can a B200 do the random 16-byte codebook gathers of the 1x16 AQLM scheme?
+// Microbenchmark: how fast can an H100 do the random 16-byte codebook gathers of the 1x16 AQLM scheme?
 //
 // Every variant streams the same packed uint16 codes (coalesced 16-byte loads, 8 codes per lane per step,
 // exactly like the GEMV kernel) and gathers one 16-byte vector per code from a 65536-entry (1 MiB) table
 // through a different path.  Output: one JSON line per variant with G gathers/s and the equivalent
 // code-bytes GB/s (2 B per gather), to be compared with the HBM roofline of the code stream.
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o tools/bin/gather_microbench tools/gather_microbench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o tools/bin/gather_microbench tools/gather_microbench.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>

@@ -9,7 +9,7 @@ benchmark/generate_benchmark.py:67-106: a Llama-architecture model whose ONE dec
                                   as notebooks/aqlm_cuda_graph.ipynb, without torch.compile).
 
 `--impl ours` uses aqlm_b200 aliased as `aqlm` (optionally with q/k/v and gate/up grouped launches, `--fuse`);
-`--impl reference` imports the UNMODIFIED reference from baseline/_ref (its CUDA kernels are JIT-built for sm_100);
+`--impl reference` imports the UNMODIFIED reference from oracle/_ref (its CUDA kernels are JIT-built for sm_90);
 `--impl dense` is the fp16 nn.Linear model.  Run each impl in its own process (both packages register `aqlm::` ops).
 One JSON line per mode on stdout.
 """
@@ -139,11 +139,11 @@ def main():
     args = ap.parse_args()
 
     if args.impl == "reference":
-        sys.path.insert(0, os.path.join(REPO, "baseline", "_ref"))
-        os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+        sys.path.insert(0, os.path.join(REPO, "oracle", "_ref"))
+        os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0")
         import aqlm
 
-        assert "baseline/_ref" in aqlm.__file__, aqlm.__file__
+        assert "oracle/_ref" in aqlm.__file__, aqlm.__file__
     elif args.impl == "ours":
         sys.path.insert(0, REPO)
         import aqlm_b200

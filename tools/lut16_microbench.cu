@@ -6,7 +6,7 @@
 // (SM, j) pair must ingest the whole 1 MiB codebook to build its LUT.  Two rates decide whether it can win:
 //   (1) random 2-byte shared-memory lookups per clock per SM (128 KiB table)     -- needs >= 6 / clk / SM
 //   (2) codebook ingest per SM in bytes/clk when a cluster shares the stream by TMA multicast -- needs >= 100 B/clk/SM
-// One JSON line per variant.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/bin/lut16_microbench tools/lut16_microbench.cu
+// One JSON line per variant.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/bin/lut16_microbench tools/lut16_microbench.cu
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,4 +1,4 @@
-"""GEMM experiment probe: for each (shape, batch) and each environment setting, check the fused dequant + tcgen05 GEMM
+"""GEMM experiment probe: for each (shape, batch) and each environment setting, check the fused dequant + wgmma GEMM
 against the C oracle (row sample) and time it (CUDA-graph replay over rotating weight copies, CUDA events).
     python tools/probe_gemm.py [--shapes 4096x14336,4096x4096] [--batches 256] [--settings "A=1,B=2;A=0"] [--scheme 1x16]
 Each setting is a ';'-separated list of comma-separated ENV=VALUE pairs (AQLM_B200_ prefix added)."""
@@ -15,7 +15,7 @@ sys.path.insert(0, os.path.join(REPO, "tests"))
 from aqlm_b200 import _cabi  # noqa: E402
 from aqlm_b200.inference_kernels import cuda_kernel  # noqa: E402
 
-KEYS = ["PDL", "GEMM_A_STAGES", "GEMM_GROUPS", "GEMM_ATMEM", "GEMM_TILE_M", "GEMM_KSPLIT", "GEMM_STAGES", "GEMM_V2", "GEMM_GATHER_MODE", "GEMM_DEBUG", "GEMM_CLUSTER"]
+KEYS = ["PDL", "GEMM_TILE_M", "GEMM_KSPLIT", "GEMM_STAGES", "GEMM_GATHER_MODE"]
 
 
 def timed(fns, iters=10):

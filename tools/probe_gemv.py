@@ -14,7 +14,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from aqlm_b200 import _cabi  # noqa: E402
 from aqlm_b200.inference_kernels import cuda_kernel  # noqa: E402
 
-L2_BYTES = 126 * 2**20
+L2_BYTES = 50 * 2**20  # H100 SXM
 
 
 def peak_gbs():

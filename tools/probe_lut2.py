@@ -27,9 +27,9 @@ def dense_ref(x, codes, codebooks, scales):
 def main():
     dev = "cuda:0"
     shapes = ((2, (4096, 11008)), (2, (4096, 4096)), (1, (4096, 11008)), (2, (4096, 22016)), (2, (4096, 12288)), (2, (1024, 4096)), (1, (4096, 4096)))
-    variants = (("shipped default (second form up to 768-row blocks, first form above)", {}),
+    variants = (("shipped default (second form, 16-row warp batches)", {}),
                 ("first form", {"AQLM_B200_LUT_CLUSTER": "1"}),
-                ("second form, auto", {"AQLM_B200_LUT_CLUSTER": "2"}),
+                ("second form", {"AQLM_B200_LUT_CLUSTER": "2"}),
                 ("second form, RB16", {"AQLM_B200_LUT_CLUSTER": "2", "AQLM_B200_LUT_C2_RB": "16"}),
                 ("second form, RB32", {"AQLM_B200_LUT_CLUSTER": "2", "AQLM_B200_LUT_C2_RB": "32"}))
     for K, (fin, fout) in shapes:

@@ -1,7 +1,7 @@
 """Opcode histogram per kernel of the shipped library (cuobjdump -sass), written as a small markdown table: the evidence
-that the tcgen05 / TMEM / TMA paths are what the .so contains (UTCHMMA = tcgen05.mma, UTMALDG = TMA tensor load, LDTM/STTM =
-tcgen05.ld/st, UTCBAR = tcgen05.commit, SYNCS = mbarrier, HMMA = mma.sync).  Runs on CPU (no GPU needed).
-    python tools/sass_summary.py > profiles/r02/sass_summary.md"""
+that the wgmma / TMA paths are what the .so contains (HGMMA = wgmma.mma_async, UTMALDG = TMA tensor load, SYNCS = mbarrier,
+HMMA = mma.sync).  Runs on CPU (no GPU needed).
+    python tools/sass_summary.py > sass_summary.md"""
 import collections
 import os
 import re
@@ -10,7 +10,7 @@ import sys
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(REPO, "aqlm_b200", "csrc", "libaqlm_b200.so")
-KEY = ["UTCHMMA", "UTMALDG", "UTMAPF", "LDTM", "STTM", "UTCBAR", "UTCATOMSWS", "SYNCS", "HMMA", "LDG", "LDS", "STS", "LDGSTS", "SHFL", "FFMA",
+KEY = ["HGMMA", "UTMALDG", "UTMAPF", "SYNCS", "HMMA", "LDG", "LDS", "STS", "LDGSTS", "SHFL", "FFMA",
        "FADD", "PRMT", "ATOMG", "MEMBAR", "ACQBULK", "UCGABAR_ARV", "BAR"]
 
 
@@ -40,7 +40,7 @@ def main():
         short = re.sub(r"^void aqlm_b200::", "", d)
         short = re.sub(r"\(.*$", "", short)
         agg[short] = c
-    print("# SASS opcode summary of aqlm_b200/csrc/libaqlm_b200.so (sm_100a)\n")
+    print("# SASS opcode summary of aqlm_b200/csrc/libaqlm_b200.so (sm_90a)\n")
     print("`python tools/sass_summary.py` (cuobjdump -sass; counts are static instruction counts per kernel instantiation).\n")
     total = collections.Counter()
     for c in agg.values():
