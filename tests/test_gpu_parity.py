@@ -286,6 +286,8 @@ def test_cuda_graph_capture_and_replay():
 
 
 # ---- fused dequant + wgmma GEMM (large batch) -----------------------------------------------------------------
+# The test_tcgen05_gemm_* names predate the Hopper port and are kept so that the test ids stay stable; they test the
+# wgmma kernels of csrc/gemm_wgmma.cuh.  Bit-exact checks of every plan are in test_zz_gemm_exact.py.
 @pytest.mark.parametrize("K,nbits", [(1, 16), (2, 8), (8, 8), (1, 8)])
 @pytest.mark.parametrize("batch", [7, 16, 64, 100, 256, 300])
 def test_tcgen05_gemm_vs_oracle_small(K, nbits, batch):
@@ -381,7 +383,8 @@ def _transposed_ref(t, go):
 def test_transposed_gemm_vs_oracle_small(K, nbits, batch):
     from aqlm_b200.inference_kernels import cuda_kernel
 
-    fin, fout = (512, 200) if batch != 64 else (1152, 456)  # ragged in both dims: in % 128 != 0, out % 64 != 0
+    # ragged in out only (out % 64 != 0); in is a multiple of 128 in both shapes -- test_zz_gemm_exact covers ragged in
+    fin, fout = (512, 200) if batch != 64 else (1152, 456)
     t = gpu_case(fin, fout, K, nbits, 1, seed=8300 + K + nbits + batch)
     go = torch.randn((batch, fout), dtype=torch.float16, device=DEV)
     before = aqlm_launches()
