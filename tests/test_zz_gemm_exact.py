@@ -37,7 +37,7 @@ gpu = pytest.mark.gpu
 
 CB_MAX, X_MAX, B_MAX = 2, 3, 8
 E_SPAN = 3                           # e_hi - e_lo: scales take 4 different values
-WS_COUNTERS = 65536                  # counter region at the head of every workspace (capi.cu kWsCountersBytes)
+WS_COUNTERS = 65536                  # counter region at the head of every workspace (plan.cuh kWsCountersBytes)
 WS_TICKETS = 8192 * 4                # its split-K ticket words; the LUT GEMV's generation words (monotonic) follow
 FINITE_MAX = {torch.float16: 65504.0, torch.bfloat16: float(torch.finfo(torch.bfloat16).max)}
 INT_EXACT = {torch.float16: 2048, torch.bfloat16: 256}  # every integer up to this is exact in the type
@@ -171,7 +171,7 @@ def assert_exact(y, ref, what, tile_m=None, n_tile=None, row_tile=128):
     pytest.fail("\n".join(lines))
 
 
-# ---- plan arithmetic (capi.cu gemm_plan / gemm_t_plan) --------------------------------------------------------------
+# ---- plan arithmetic (plan.cuh gemm_plan / gemm_t_plan) ------------------------------------------------------------
 def n_tile_of(batch):
     n = 16
     while n < 128 and n < batch:
