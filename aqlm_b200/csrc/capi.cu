@@ -210,26 +210,19 @@ static size_t vec_smem_bytes(const GemvParams& p, int K, int code_bytes, int G, 
          (size_t)rows_cta * slices * BT * 4;
 }
 
-template <typename T, int K, int CB, int G, int BT, bool CBS, int GM>
+template <typename T, int K, int CB, int G, int BT, bool CBS>
 static int launch_vec(const GemvParams& p, const DeviceInfo* di, cudaStream_t st) {
   constexpr int THREADS = (BT <= 2) ? 1024 : 512;
   const int grid = di->sm_count * tun().gemv_ctas_per_sm;
-  return launch<gemv_vec_kernel<T, K, CB, G, BT, CBS, GM, THREADS>>(di, grid, THREADS,
-                                                                    vec_smem_bytes(p, K, CB, G, BT, CBS, grid), st, 0, p);
+  return launch<gemv_vec_kernel<T, K, CB, G, BT, CBS, THREADS>>(di, grid, THREADS,
+                                                                vec_smem_bytes(p, K, CB, G, BT, CBS, grid), st, 0, p);
 }
 
-// 512-thread CTAs, one per SM (default), or 256-thread CTAs, two per SM (AQLM_B200_GEMV_THREADS=256; batch 1 only)
-template <typename T, int BT, int GM>
+template <typename T, int BT>
 static int launch_1x16(const GemvParams& p, const DeviceInfo* di, cudaStream_t st) {
-  const auto go = [&](auto THREADS) {
-    const int grid = di->sm_count * (512 / THREADS);
-    return launch<gemv_1x16_kernel<T, BT, GM, THREADS>>(di, grid, THREADS, vec_smem_bytes(p, 1, 2, 8, BT, false, grid),
-                                                        st, 0, p, GemvPeer{});
-  };
-  if constexpr (BT == 1 && GM == 0) {
-    if (tun().gemv_threads == 256) return go(Int<256>{});
-  }
-  return go(Int<kGemv1x16Threads>{});
+  const int grid = di->sm_count;
+  return launch<gemv_1x16_kernel<T, BT>>(di, grid, kGemv1x16Threads, vec_smem_bytes(p, 1, 2, 8, BT, false, grid), st, 0,
+                                         p, GemvPeer{});
 }
 
 // Fused GEMV + peer-memory exchange (gemv_1x16_kernel<..., PEER = true>): contiguous row blocks, one CTA per SM.
@@ -245,7 +238,7 @@ static int launch_1x16_peer(GemvParams p, const GemvPeer& pc, const DeviceInfo* 
   const size_t smem = (size_t)BT * p.in_features * 2 + (size_t)rb * slices * BT * 4;
   if (smem > (size_t)di->max_smem_optin - 1024)
     return fail(AQLM_B200_ERR_UNSUPPORTED, "fused exchange: activation tile + partials do not fit in shared memory");
-  return launch<gemv_1x16_kernel<T, BT, 0, kGemv1x16Threads, true>>(di, grid, kGemv1x16Threads, smem, st, 0, p, pc);
+  return launch<gemv_1x16_kernel<T, BT, true>>(di, grid, kGemv1x16Threads, smem, st, 0, p, pc);
 }
 
 template <typename T, int CB, int G, int BT>
@@ -269,26 +262,17 @@ static int dispatch_bt(const aqlm_b200_weight_t* w, const GemvParams& p, const D
   const int grid = di->sm_count * tun().gemv_ctas_per_sm;
   const bool pow2k = (K == 1 || K == 2 || K == 4 || K == 8);
   const size_t need = pow2k ? vec_smem_bytes(p, K, code_bytes, G, BT, nbits == 8, grid) : (size_t)-1;
-  if (vec_ok && nbits == 16 && K == 1 && need <= budget) {
-    const int gm = tun().gather_mode;
-    if (G == 8 && tun().gemv_v2 && vec_smem_bytes(p, 1, 2, 8, BT, false, di->sm_count) <= budget) {
-      if (gm == 1) return launch_1x16<T, BT, 1>(p, di, st);
-      return launch_1x16<T, BT, 0>(p, di, st);
-    }
-    if (G == 8) {
-      if (gm == 1) return launch_vec<T, 1, 2, 8, BT, false, 1>(p, di, st);
-      if (gm == 2) return launch_vec<T, 1, 2, 8, BT, false, 2>(p, di, st);
-      return launch_vec<T, 1, 2, 8, BT, false, 0>(p, di, st);
-    }
-    // g = 16: one codebook entry is fetched as ONE 256-bit request, which needs a 32-byte aligned table (any torch
-    // allocation is); a 16-byte aligned table handed in through the C-ABI takes the generic kernel below
-    if ((reinterpret_cast<uintptr_t>(w->codebooks) & 31) == 0) return launch_vec<T, 1, 2, 16, BT, false, 0>(p, di, st);
-  }
+  if (vec_ok && nbits == 16 && K == 1 && G == 8 && vec_smem_bytes(p, 1, 2, 8, BT, false, di->sm_count) <= budget)
+    return launch_1x16<T, BT>(p, di, st);
+  // g = 16: one codebook entry is fetched as ONE 256-bit request, which needs a 32-byte aligned table (any torch
+  // allocation is); a 16-byte aligned table handed in through the C-ABI takes the generic kernel below
+  if (vec_ok && nbits == 16 && K == 1 && G == 16 && need <= budget && (reinterpret_cast<uintptr_t>(w->codebooks) & 31) == 0)
+    return launch_vec<T, 1, 2, 16, BT, false>(p, di, st);
   if (vec_ok && nbits == 8 && G == 8 && pow2k && need <= budget) {
-    if (K == 1) return launch_vec<T, 1, 1, 8, BT, true, 0>(p, di, st);
-    if (K == 2) return launch_vec<T, 2, 1, 8, BT, true, 0>(p, di, st);
-    if (K == 4) return launch_vec<T, 4, 1, 8, BT, true, 0>(p, di, st);
-    if (K == 8) return launch_vec<T, 8, 1, 8, BT, true, 0>(p, di, st);
+    if (K == 1) return launch_vec<T, 1, 1, 8, BT, true>(p, di, st);
+    if (K == 2) return launch_vec<T, 2, 1, 8, BT, true>(p, di, st);
+    if (K == 4) return launch_vec<T, 4, 1, 8, BT, true>(p, di, st);
+    if (K == 8) return launch_vec<T, 8, 1, 8, BT, true>(p, di, st);
   }
   if (code_bytes == 2) {
     if (G == 8) return launch_generic<T, 2, 8, BT>(p, di, st);
@@ -355,7 +339,6 @@ static int launch_lut(const aqlm_b200_weight_t* w, const void* input, void* outp
   p.n_slabs = L.n_slabs;
   p.rows_per_block = L.rows_per_block;
   p.partial_f32 = (flags & AQLM_B200_FLAG_PARTIAL_F32) ? 1 : 0;
-  p.debug = tun().lut_debug;
   constexpr int THREADS = (K <= 2) ? 256 : 512;  // K >= 4: one CTA per SM (128 KiB LUT), so give it 16 warps
   return launch<gemv_lut_kernel<T, K, J, THREADS>>(di, dim3(L.n_slabs, L.row_blocks), THREADS, L.smem, st, 0, p);
 }
@@ -388,31 +371,20 @@ static LutClusterParams lut_cluster_params(const aqlm_b200_weight_t* w, const vo
   return p;
 }
 
-// Second form of the cluster kernel (gemv_lut_cluster2_kernel): LUT at absolute shared address 0x10000, one warp per
-// row batch (the CTA size follows the row block), push-based cross-slab sum.
-template <typename T, int K, int RB, int MAXT = 1024>
-static int launch_lut_cluster2(const LutClusterParams& p, int row_blocks, const DeviceInfo* di, cudaStream_t st) {
-  int warps = (p.rows_per_block + RB - 1) / RB;
-  warps = warps < 8 ? 8 : (warps > 32 ? 32 : warps);
-  if (MAXT == 1024 && warps <= 24)  // <= 768 threads: the 80-register build (the 64-register one spills ~50 words at RB = 32)
-    return launch_lut_cluster2<T, K, RB, 768>(p, row_blocks, di, st);
-  const size_t smem = (size_t)kLutAbs + (size_t)K * 256 * kLutCJ * 4;  // LUT ends at 0x10000 * (1 + K) whatever the window base
-  return launch<gemv_lut_cluster2_kernel<T, K, RB, MAXT>>(di, dim3(p.n_slabs, row_blocks), warps * 32, smem, st,
-                                                          p.n_slabs, p);
-}
-
 // ---- Kx8 LUT GEMV, cluster / DSMEM variant (K <= 2, at most 8 slabs of 64 groups): host side ---------------
-template <typename T, int K, int RB, int THREADS>
+template <typename T, int K>
 static int launch_lut_cluster(const aqlm_b200_weight_t* w, const void* input, void* output, uint32_t flags,
                               const DeviceInfo* di, cudaStream_t st, bool* taken) {
   *taken = false;
   const int n_slabs = lut_cluster_slabs(*w);
-  constexpr auto kernel = gemv_lut_cluster_kernel<T, K, RB, THREADS>;
   const size_t lut_bytes = (size_t)K * 256 * kLutCJ * 4;
-  // how many clusters of n_slabs CTAs can be resident at once (the second form's grid is sized from this query too)
+  // How many clusters of n_slabs CTAs can be resident at once; the grid is sized from this.  The query describes
+  // 512-thread CTAs with the LUT + 8 KiB of shared memory, not the launch below: at 512 threads the 768-thread build's
+  // registers allow one CTA per SM, as the launch's shared memory does.
   static std::atomic<int> max_clusters[kMaxDevices][9];
   int mc = max_clusters[di->index][n_slabs].load(std::memory_order_relaxed);
   if (mc == 0) {
+    constexpr auto kernel = gemv_lut_cluster_kernel<T, K, 768>;
     const size_t smem_max = lut_bytes + 8192;
     if (int rc = ensure_smem<kernel>(smem_max, di)) return rc;
     cudaLaunchAttribute attr[1];
@@ -422,7 +394,7 @@ static int launch_lut_cluster(const aqlm_b200_weight_t* w, const void* input, vo
     attr[0].val.clusterDim.z = 1;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(n_slabs, di->sm_count);
-    cfg.blockDim = dim3(THREADS);
+    cfg.blockDim = dim3(512);
     cfg.dynamicSmemBytes = smem_max;
     cfg.stream = st;
     cfg.attrs = attr;
@@ -438,15 +410,15 @@ static int launch_lut_cluster(const aqlm_b200_weight_t* w, const void* input, vo
   const LutClusterRows r = lut_cluster_rows(*w, mc);
   if (!r.rows_per_block) return AQLM_B200_OK;
   const LutClusterParams p = lut_cluster_params(w, input, output, flags, n_slabs, r.rows_per_block);
-  int rc;
-  if (tun().lut_cluster >= 2) {  // second form: same grid / cluster shape, its own CTA size and shared-memory map
-    const int rb_sel = tun().lut_c2_rb ? tun().lut_c2_rb : 16;
-    rc = rb_sel == 16 ? launch_lut_cluster2<T, K, 16>(p, r.row_blocks, di, st)
-                      : launch_lut_cluster2<T, K, 32>(p, r.row_blocks, di, st);
-  } else {
-    rc = launch<kernel>(di, dim3(n_slabs, r.row_blocks), THREADS, lut_bytes + (size_t)r.rows_per_block * 4, st,
-                        n_slabs, p);
-  }
+  // one warp per 16-row batch of the row block (8 to 32 warps); up to 768 threads the 80-register build
+  int warps = (r.rows_per_block + 15) / 16;
+  warps = warps < 8 ? 8 : (warps > 32 ? 32 : warps);
+  const size_t smem = (size_t)kLutAbs + lut_bytes;  // LUT ends at 0x10000 * (1 + K) whatever the window base
+  const auto go = [&](auto MAXT) {
+    return launch<gemv_lut_cluster_kernel<T, K, MAXT>>(di, dim3(n_slabs, r.row_blocks), warps * 32, smem, st, n_slabs,
+                                                       p);
+  };
+  const int rc = warps <= 24 ? go(Int<768>{}) : go(Int<1024>{});
   *taken = rc == AQLM_B200_OK;
   return rc;
 }
@@ -458,11 +430,8 @@ static int try_lut_cluster(const aqlm_b200_weight_t* w, const void* input, void*
   if (!lut_cluster_eligible(*w, input, batch, tun())) return AQLM_B200_OK;
   return with_dtype(w->dtype, [&](auto tag) {
     using T = typename decltype(tag)::type;
-    const auto go = [&](auto K) {
-      return tun().lut_rb16 ? launch_lut_cluster<T, K, 16, 768>(w, input, output, flags, di, st, taken)
-                            : launch_lut_cluster<T, K, 32, kLutCThreads>(w, input, output, flags, di, st, taken);
-    };
-    return w->num_codebooks == 1 ? go(Int<1>{}) : go(Int<2>{});
+    return w->num_codebooks == 1 ? launch_lut_cluster<T, 1>(w, input, output, flags, di, st, taken)
+                                 : launch_lut_cluster<T, 2>(w, input, output, flags, di, st, taken);
   });
 }
 
@@ -664,7 +633,7 @@ int aqlm_b200_matmat_ws(const aqlm_b200_weight_t* w, const void* input, void* ou
       if (rc || taken) return rc;
     }
     const LutPlan L = lut_plan(*w, 1, *di, tun());
-    const bool cluster_case = w->num_codebooks <= 2 && (w->in_features / 8) <= 8 * kLutCJ && tun().lut_cluster;
+    const bool cluster_case = w->num_codebooks <= 2 && (w->in_features / 8) <= 8 * kLutCJ;
     if (L.ok && workspace_bytes >= kWsCountersBytes + L.partials_bytes && !(batch > 1 && cluster_case)) {
       const size_t out_elt = partial ? 4 : 2;
       for (int64_t b = 0; b < ws_rows; ++b) {  // launches are stream-ordered: the workspace is reused row after row
@@ -710,7 +679,7 @@ int aqlm_b200_matmat_grouped(const aqlm_b200_weight_t* w, const int64_t* seg_row
   return with_batch_tile(batch, [&](auto BT) {
     if (vec_smem_bytes(p, 1, 2, 8, BT, false, di->sm_count) > (size_t)di->max_smem_optin - 1024)
       return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped launch: activation tile does not fit in shared memory");
-    return with_dtype(w->dtype, [&](auto tag) { return launch_1x16<typename decltype(tag)::type, BT, 0>(p, di, st); });
+    return with_dtype(w->dtype, [&](auto tag) { return launch_1x16<typename decltype(tag)::type, BT>(p, di, st); });
   });
 }
 

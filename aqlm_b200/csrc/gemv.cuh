@@ -54,7 +54,6 @@ constexpr int kSliceChunks = 32;   // one K-slice = 32 16-byte code chunks = one
 //   T          __half | __nv_bfloat16
 //   K          codebooks per group;  CODE_BYTES 1|2;  G in_group_size (8|16);  BT batch rows per pass
 //   CBS        codebooks staged in shared memory (256-entry codebooks) vs gathered from global/L2 (1x16)
-//   GM         gather flavour for the global path (see ld_gather_v4)
 //   THREADS    CTA size; the grid is persistent: (SM count) x (CTAs per SM that fit)
 //
 // Work decomposition (load balance is what matters: the kernel is bound by the per-SM gather rate, so every
@@ -64,7 +63,7 @@ constexpr int kSliceChunks = 32;   // one K-slice = 32 16-byte code chunks = one
 // CTA adds the slices of each of its rows IN A FIXED ORDER (deterministic, batch-invariant) and applies
 // scale + bias.  No atomics, no second launch.
 // ---------------------------------------------------------------------------------------------------
-template <typename T, int K, int CODE_BYTES, int G, int BT, bool CBS, int GM, int THREADS>
+template <typename T, int K, int CODE_BYTES, int G, int BT, bool CBS, int THREADS>
 __global__ void __launch_bounds__(THREADS, 1) gemv_vec_kernel(const GemvParams p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   constexpr int GPC = 16 / (K * CODE_BYTES);  // groups per 16-byte chunk
@@ -139,12 +138,12 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_vec_kernel(const GemvParams p
         for (int e = 0; e < GPC; ++e) {
           const uint32_t code = chunk_code<CODE_BYTES>(cw, e);
           if constexpr (!CBS && UPG == 2) {  // g = 16: the 32-byte entry is one 256-bit request
-            ld_gather_v8<GM>(gcb + (size_t)code * 2, wv[e][0], wv[e][1]);
+            ld_gather_v8(gcb + (size_t)code * 2, wv[e][0], wv[e][1]);
           } else {
 #pragma unroll
             for (int h = 0; h < UPG; ++h) {
               if constexpr (CBS) wv[e][h] = scb[code * UPG + h];
-              else wv[e][h] = ld_gather_v4<GM>(gcb + (size_t)code * UPG + h);
+              else wv[e][h] = ld_gather_v4<0>(gcb + (size_t)code * UPG + h);
             }
           }
         }
@@ -169,7 +168,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_vec_kernel(const GemvParams p
             for (int h = 0; h < UPG; ++h) {
               uint4 v;
               if constexpr (CBS) v = scb[off + h];
-              else v = ld_gather_v4<GM>(gcb + off + h);
+              else v = ld_gather_v4<0>(gcb + off + h);
               if (k == 0) unpack8<T>(v, wf[h]);
               else accum8<T>(v, wf[h]);
             }
@@ -226,9 +225,10 @@ constexpr int kGemv1x16Threads = 512;
 //   fence, flag or barrier in between (see the epilogue).  A thread only ever waits for the same element of the other ranks.
 // Two buffer sets alternate by step parity; `step` is read after griddepcontrol.wait (the previous launch, which
 // advances it, has completed).  The grid is one CTA per SM, all co-resident, so the cross-rank wait cannot deadlock.
-template <typename T, int BT, int GM, int THREADS = kGemv1x16Threads, bool PEER = false>
-__global__ void __launch_bounds__(THREADS, 512 / THREADS) gemv_1x16_kernel(const GemvParams p, const GemvPeer pc) {
+template <typename T, int BT, bool PEER = false>
+__global__ void __launch_bounds__(kGemv1x16Threads, 1) gemv_1x16_kernel(const GemvParams p, const GemvPeer pc) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
+  constexpr int THREADS = kGemv1x16Threads;
   constexpr int kWarps = THREADS / 32;
   const int upr = p.in_features >> 3;
   griddep_launch_dependents();
@@ -268,7 +268,7 @@ __global__ void __launch_bounds__(THREADS, 512 / THREADS) gemv_1x16_kernel(const
   auto gather = [&](int t, const uint4& cw, uint4 (&w)[8]) {
     const uint4* cb = task_codebook(t);
 #pragma unroll
-    for (int e = 0; e < 8; ++e) w[e] = ld_gather_v4<GM>(cb + chunk_code<2>(cw, e));
+    for (int e = 0; e < 8; ++e) w[e] = ld_gather_v4<0>(cb + chunk_code<2>(cw, e));
   };
   auto consume = [&](int t, bool live, const uint4 (&w)[8]) {
     float acc[BT];

@@ -37,7 +37,6 @@ struct LutParams {
   int n_slabs;
   int rows_per_block;  // multiple of 32
   int partial_f32;
-  int debug;           // experiments: bit0 skip the lookup phase, bit1 skip the LUT build, bit2 skip partials + fix-up
 };
 
 
@@ -127,7 +126,9 @@ __global__ void __launch_bounds__(kLutThreads, (kLutThreads == 256) ? 2 : 1) gem
   griddep_wait();  // x is produced by the previous kernel
 
   // ---------------- LUT build: D[16 entries x 8 groups] = CB[16 x 8] . X^T[8 x 8], tensor cores ----------------
-  if (!(p.debug & 2)) {
+  // The host launches no empty slab, so the guard always holds.  It keeps ptxas from scheduling the build together with
+  // the lookups: for K = 8 that costs one extra instruction per lookup and ~3% of the 8x8 GEMV's time on an H100.
+  if (j0 < p.in_groups) {
     // column (2m'+i) of n-tile t holds group (2*NT)*m' + 2t + i, so a lane ends up with 2*NT consecutive groups
     uint32_t bfrag[NT];
 #pragma unroll
@@ -202,13 +203,10 @@ __global__ void __launch_bounds__(kLutThreads, (kLutThreads == 256) ? 2 : 1) gem
     const int row = rbase + jj * RPW + rsub;
     if (row < row_end) part[row] = v[0];
   };
-  if (!(p.debug & 1)) {
-    for (; r0 < row_end; r0 += 2 * kBatchStride) {
-      process(r0, cwa);
-      if (r0 + kBatchStride < row_end) process(r0 + kBatchStride, cwb);
-    }
+  for (; r0 < row_end; r0 += 2 * kBatchStride) {
+    process(r0, cwa);
+    if (r0 + kBatchStride < row_end) process(r0 + kBatchStride, cwb);
   }
-  if (p.debug & 4) return;
 
   // ---------------- fix-up: ALL slab CTAs of this row block share the cross-slab sum ----------------
   // The grid is one resident wave (host side guarantees it), so the n_slabs CTAs of a row block can rendezvous: each
@@ -262,14 +260,27 @@ __global__ void __launch_bounds__(kLutThreads, (kLutThreads == 256) ? 2 : 1) gem
 
 // ---------------------------------------------------------------------------------------------------
 // Cluster variant for K = 1, 2 and in_features <= 8 slabs of 64 groups (4096 for g = 8): the slab CTAs of a row block form
-// ONE thread-block cluster and reduce their partial rows through DISTRIBUTED SHARED MEMORY -- no global partials, no
-// fence/atomic/poll round trips through global memory.
-//   * slab = 64 in-groups, LUT [K][256][64] fp32 (64/128 KiB), 512 threads, one CTA per SM;
+// ONE thread-block cluster and reduce their partial rows through DISTRIBUTED SHARED MEMORY -- no workspace, no global
+// partials, no fence/atomic/poll round trips through global memory.  One CTA per SM.
+//   * slab = 64 in-groups, LUT [K][256][64] fp32 (64/128 KiB), built by tensor cores as in gemv_lut_kernel.  A LUT row
+//     (one entry, 64 groups) is 256 bytes.
 //   * a lane owns the ADJACENT groups 2l, 2l+1: one aligned code word per row (K=2: 4 bytes, K=1: 2 bytes) = a fully
-//     coalesced 128/64-byte row segment per warp; group 2l sits at LUT position l, group 2l+1 at position 32+l, so both
-//     lookups of a lane hit bank l (conflict-free) and the row stride is 256 B: byte 1 of the word is already a row offset;
-//   * per-row totals of the slab go to shared memory; after a cluster barrier CTA r adds, IN SLAB ORDER (deterministic),
-//     the n_slabs partial values of every row of its share with ld.shared::cluster, applies scale + bias and writes y.
+//     coalesced 128/64-byte row segment per warp.  Group 2l sits at LUT position l and group 2l+1 at position 32+l, so
+//     both lookups of a lane hit bank l: the lookups never conflict.
+//   * ONE instruction of address arithmetic per lookup.  The LUT is placed at the first 64 KiB boundary of the CTA's
+//     shared window above the receive buffers (window offset 0x10000; codebook k at 0x10000 * (1 + k)), so the address of
+//     entry `code` for the lane's even group is  {byte3, byte2, byte1, byte0} = {base.hi, base.lo + k, code, 4 * lane}:
+//     one PRMT takes the code byte straight out of the packed code word and the other three bytes from a per-lane
+//     constant; the odd group is the immediate offset +128 of the LDS.  The ~63 KiB below 0x10000 are not wasted on this
+//     1-CTA/SM kernel: they hold the receive buffers of the cross-slab sum.
+//   * every warp owns ONE batch of 16 rows: the CTA is launched with as many warps as its row block has batches (8 to 32,
+//     MAXT = 768 or 1024 threads), so there is no second, mostly empty, round and nothing is double-buffered.  16 rows
+//     over 32 lanes: the two half-warps are folded first, then a 15-shuffle transpose-reduce over 16 lanes leaves lane l
+//     with the slab total of row l of the batch.
+//   * the cross-slab sum is PUSH-based: a lane that holds the slab total of a row stores it (st.shared::cluster) into the
+//     receive buffer of the CTA that owns the row's share; after ONE cluster barrier every CTA adds the n_slabs values of
+//     its rows from its OWN shared memory, in slab order (deterministic).  No remote loads, no second barrier (nobody
+//     touches a peer's memory after the barrier).
 // ---------------------------------------------------------------------------------------------------
 struct LutClusterParams {
   const void* codes;
@@ -286,199 +297,12 @@ struct LutClusterParams {
 };
 
 constexpr int kLutCJ = 64;
-constexpr int kLutCThreads = 512;
-
-__device__ __forceinline__ float ld_dsmem_f32(uint32_t local_smem_addr, uint32_t cta_rank) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local_smem_addr), "r"(cta_rank));
-  float v;
-  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(remote) : "memory");
-  return v;
-}
-
-// RB = rows per warp batch (32: one butterfly of 31 shuffles per 32 rows; 16: 31 shuffles per 16 rows but twice as many,
-// smaller batches to deal to 24 warps -- the row block of a cluster is only ~700 rows = 22 batches of 32).
-template <typename T, int K, int RB = 32, int THREADS = kLutCThreads>
-__global__ void __launch_bounds__(THREADS, 1) gemv_lut_cluster_kernel(const LutClusterParams p) {
-  static_assert(K == 1 || K == 2, "cluster LUT kernel: one or two 256-entry codebooks");
-  static_assert(RB == 32 || RB == 16, "rows per warp batch");
-  extern __shared__ __align__(16) float lut[];  // [K][256][64], then spart[rows_per_block]
-  constexpr int J = kLutCJ, NT = J / 8, kWarps = THREADS / 32;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int slab = blockIdx.x, rb = blockIdx.y;
-  const int j0 = slab * J;
-  griddep_launch_dependents();
-  float* spart = lut + (size_t)K * 256 * J;
-  const int row_begin = rb * p.rows_per_block;
-  const int row_end = min(p.out_features, row_begin + p.rows_per_block);
-  const size_t row_bytes = (size_t)p.in_groups * K;
-  // lane <-> groups (j0 + 2l, j0 + 2l + 1): CW = 2K code bytes per row
-  using CodeWord = typename std::conditional<K == 2, uint32_t, uint16_t>::type;
-  const bool g_ok = j0 + 2 * lane + 1 < p.in_groups;   // (in_groups is even for every shape this kernel accepts)
-  const uint8_t* cbase = reinterpret_cast<const uint8_t*>(p.codes) + (size_t)(j0 + 2 * lane) * K;
-  constexpr int kBatchStride = kWarps * RB;
-  auto load_codes = [&](int r0, uint32_t (&cw)[RB]) {
-    const uint8_t* src = cbase + (size_t)r0 * row_bytes;
-    if (g_ok && r0 + RB <= row_end) {
-#pragma unroll
-      for (int i = 0; i < RB; ++i, src += row_bytes) cw[i] = (uint32_t)__ldg(reinterpret_cast<const CodeWord*>(src));
-    } else {
-#pragma unroll
-      for (int i = 0; i < RB; ++i, src += row_bytes) {
-        cw[i] = 0u;
-        if (g_ok && r0 + i < row_end) cw[i] = (uint32_t)__ldg(reinterpret_cast<const CodeWord*>(src));
-      }
-    }
-  };
-  // ---- prologue (weights only; overlaps the previous kernel under PDL) ----
-  uint32_t cwa[RB], cwb[RB];
-  int r0 = row_begin + warp * RB;
-  load_codes(r0, cwa);
-  if (r0 + kBatchStride < row_end) load_codes(r0 + kBatchStride, cwb);
-  constexpr int MT = (K * 16 + kWarps - 1) / kWarps;  // 16-entry tiles per warp (the last pass may be partial)
-  const int q = lane >> 2, m = lane & 3;
-  uint32_t afrag[MT][2];
-  {
-    const uint32_t* cb32 = reinterpret_cast<const uint32_t*>(p.codebooks);
-#pragma unroll
-    for (int u = 0; u < MT; ++u) {
-      const int tile = warp + u * kWarps;
-      const int e0 = (tile < K * 16 ? tile : 0) * 16;
-      afrag[u][0] = __ldg(cb32 + (size_t)(e0 + q) * 4 + m);
-      afrag[u][1] = __ldg(cb32 + (size_t)(e0 + q + 8) * 4 + m);
-    }
-  }
-  griddep_wait();  // x is produced by the previous kernel
-  // ---- LUT build (tensor cores): lane (q, m) ends with groups 16m .. 16m+15 of entries e0+q and e0+q+8;
-  //      even groups go to positions 8m + t, odd groups to 32 + 8m + t ----
-  {
-    uint32_t bfrag[NT];
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-      const int gg = j0 + 16 * (q >> 1) + 2 * t + (q & 1);
-      bfrag[t] = gg < p.in_groups ? reinterpret_cast<const uint32_t*>(p.x)[gg * 4 + m] : 0u;
-    }
-#pragma unroll
-    for (int u = 0; u < MT; ++u) {
-      const int tile = warp + u * kWarps;
-      if (tile >= K * 16) break;  // (warp-uniform)
-      const int e0 = tile * 16;
-      float d[NT][4];
-#pragma unroll
-      for (int t = 0; t < NT; ++t) {
-        d[t][0] = d[t][1] = d[t][2] = d[t][3] = 0.f;
-        mma_m16n8k8(d[t], afrag[u][0], afrag[u][1], bfrag[t], DT<T>::is_bf16);
-      }
-      float* ra = lut + (size_t)(e0 + q) * J + 8 * m;
-      float* rb8 = lut + (size_t)(e0 + q + 8) * J + 8 * m;
-      const bool odd = q & 1;  // odd entry rows store their second half first: a quarter-warp then covers all 32 banks
-      // c: which accumulator column (0/1: entry e0+q, even/odd groups; 2/3: entry e0+q+8)
-#define AQLM_LUT_ROW(dst, c)                                                                            \
-      {                                                                                                 \
-        const float4 lo = make_float4(d[0][c], d[1][c], d[2][c], d[3][c]);                              \
-        const float4 hi = make_float4(d[4][c], d[5][c], d[6][c], d[7][c]);                              \
-        *reinterpret_cast<float4*>((dst) + (odd ? 4 : 0)) = odd ? hi : lo;                              \
-        *reinterpret_cast<float4*>((dst) + (odd ? 0 : 4)) = odd ? lo : hi;                              \
-      }
-      AQLM_LUT_ROW(ra, 0)
-      AQLM_LUT_ROW(ra + 32, 1)
-      AQLM_LUT_ROW(rb8, 2)
-      AQLM_LUT_ROW(rb8 + 32, 3)
-#undef AQLM_LUT_ROW
-    }
-  }
-  __syncthreads();
-  // ---- lookups ----
-  const uint32_t lane_off = (uint32_t)lane * 4u;
-  const char* lut_b = reinterpret_cast<const char*>(lut);
-  auto process = [&](int rbase, uint32_t (&cw)[RB]) {
-    float v[RB];
-#pragma unroll
-    for (int i = 0; i < RB; ++i) {
-      const uint32_t w = cw[i];
-      float acc;
-      if constexpr (K == 2) {  // bytes: [g0 k0][g0 k1][g1 k0][g1 k1]; a LUT row is 256 B
-        acc = *reinterpret_cast<const float*>(lut_b + (((w << 8) & 0xff00u) | lane_off));
-        acc += *reinterpret_cast<const float*>(lut_b + 65536 + ((w & 0xff00u) | lane_off));
-        acc += *reinterpret_cast<const float*>(lut_b + 128 + (((w >> 8) & 0xff00u) | lane_off));
-        acc += *reinterpret_cast<const float*>(lut_b + 65536 + 128 + (((w >> 16) & 0xff00u) | lane_off));
-      } else {                 // bytes: [g0][g1]
-        acc = *reinterpret_cast<const float*>(lut_b + (((w << 8) & 0xff00u) | lane_off));
-        acc += *reinterpret_cast<const float*>(lut_b + 128 + ((w & 0xff00u) | lane_off));
-      }
-      v[i] = acc;
-    }
-    if (rbase + 2 * kBatchStride < row_end) load_codes(rbase + 2 * kBatchStride, cw);
-    if constexpr (RB == 16) {  // 16 rows over 32 lanes: fold the two half-warps first, then transpose-reduce over 16 lanes
-#pragma unroll
-      for (int i = 0; i < RB; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i], 16);
-    }
-#pragma unroll
-    for (int dd = (RB == 32 ? 16 : 8), n = RB; dd >= 1; dd >>= 1, n >>= 1) {
-      const bool up = (lane & dd) != 0;
-#pragma unroll
-      for (int i = 0; i < n / 2; ++i) {
-        const float send = up ? v[i] : v[i + n / 2];
-        const float keep = up ? v[i + n / 2] : v[i];
-        v[i] = keep + __shfl_xor_sync(0xffffffffu, send, dd);
-      }
-    }
-    const int row = rbase + (lane & (RB - 1));
-    if (row < row_end && lane < RB) spart[row - row_begin] = v[0];
-  };
-  for (; r0 < row_end; r0 += 2 * kBatchStride) {
-    process(r0, cwa);
-    if (r0 + kBatchStride < row_end) process(r0 + kBatchStride, cwb);
-  }
-  // ---- cross-slab sum through distributed shared memory ----
-  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-  {
-    const int nrows = row_end - row_begin;
-    const int per = (nrows + p.n_slabs - 1) / p.n_slabs;
-    const int lo = slab * per, hi = min(nrows, lo + per);
-    const uint32_t sp = (uint32_t)__cvta_generic_to_shared(spart);
-    for (int r = lo + tid; r < hi; r += THREADS) {
-      float acc = 0.f;
-      for (int s2 = 0; s2 < p.n_slabs; ++s2) acc += ld_dsmem_f32(sp + 4u * (uint32_t)r, (uint32_t)s2);
-      const int row = row_begin + r;
-      if (p.partial_f32) {
-        reinterpret_cast<float*>(p.y)[row] = acc;
-      } else {
-        const float sc = DT<T>::to_float(reinterpret_cast<const T*>(p.scales)[row]);
-        const float bi = p.bias ? DT<T>::to_float(reinterpret_cast<const T*>(p.bias)[row]) : 0.f;
-        reinterpret_cast<T*>(p.y)[row] = DT<T>::from_float(fmaf(acc, sc, bi));
-      }
-    }
-  }
-  // nobody leaves while a peer may still read its shared memory
-  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-
-// ---------------------------------------------------------------------------------------------------
-// Cluster kernel, second form (default for K <= 2, in_features <= 8 slabs of 64 groups).  Same slab / lane <-> adjacent-group
-// layout and the same tensor-core LUT build as gemv_lut_cluster_kernel; three changes, aimed at the cost of the lookups
-// and of the cross-slab sum:
-//   * ONE instruction of address arithmetic per lookup.  The LUT is placed at the first 64 KiB boundary of the CTA's
-//     shared window above the receive buffers (window offset 0x10000; codebook k at 0x10000 * (1 + k)); a LUT row (one entry, 64 groups) is 256 bytes, so the address of entry `code` for
-//     the lane's group is  {byte3, byte2, byte1, byte0} = {base.hi, base.lo + k, code, 4 * lane}  -- one PRMT that takes the code byte
-//     straight out of the packed code word and the other three bytes from a per-lane constant; the lane's second (odd) group
-//     is the immediate offset +128 of the LDS.  (The first form spent SHL + LOP3 + IADD per lookup.)  The ~63 KiB below
-//     0x10000 are not wasted on this 1-CTA/SM kernel: they hold the receive buffers of the cross-slab sum.
-//   * every warp owns ONE batch of rows: the CTA is launched with as many warps as its row block has batches (<= 32), so
-//     there is no second, mostly empty, round (22 batches on 16 warps = 2 rounds before), and nothing is double-buffered
-//     (<= 64 registers).
-//   * the cross-slab sum is PUSH-based: a lane that ends the transpose-reduce with the slab total of a row stores it
-//     (st.shared::cluster) into the receive buffer of the CTA that owns the row's share; after ONE cluster barrier every CTA
-//     adds the n_slabs values of its rows from its OWN shared memory, in slab order (deterministic).  No remote loads, no
-//     second barrier (nobody touches a peer's memory after the barrier).
-// ---------------------------------------------------------------------------------------------------
 constexpr uint32_t kLutAbs = 0x10000u;  // absolute shared-memory address of LUT 0
 
-template <typename T, int K, int RB, int MAXT>
-__global__ void __launch_bounds__(MAXT, 1) gemv_lut_cluster2_kernel(const LutClusterParams p) {
+template <typename T, int K, int MAXT>
+__global__ void __launch_bounds__(MAXT, 1) gemv_lut_cluster_kernel(const LutClusterParams p) {
   static_assert(K == 1 || K == 2, "cluster LUT kernel: one or two 256-entry codebooks");
-  static_assert(RB == 32 || RB == 16, "rows per warp batch");
+  constexpr int RB = 16;  // rows per warp batch
   extern __shared__ __align__(16) uint8_t smem_dyn[];
   constexpr int J = kLutCJ, NT = J / 8;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -548,8 +372,7 @@ __global__ void __launch_bounds__(MAXT, 1) gemv_lut_cluster2_kernel(const LutClu
 #pragma unroll
       for (int h = 0; h < 2; ++h) {  // two passes of 4 n-tiles (keeps the accumulators at 16 registers).  Every lane of a
                                      // pass holds the SAME half, so the even and the odd entry row of a quarter-warp store
-                                     // to the same banks (2-way conflict on the build stores; the first form avoids it by
-                                     // holding all 32 accumulators and letting odd rows store their second half first)
+                                     // to the same banks: a 2-way conflict on the build stores, the price of those registers
         float d[4][4];
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
@@ -590,12 +413,11 @@ __global__ void __launch_bounds__(MAXT, 1) gemv_lut_cluster2_kernel(const LutClu
         v[i] = t0 + t1;
       }
     }
-    if constexpr (RB == 16) {  // 16 rows over 32 lanes: fold the two half-warps first, then transpose-reduce over 16 lanes
+    // 16 rows over 32 lanes: fold the two half-warps first, then transpose-reduce over 16 lanes
 #pragma unroll
-      for (int i = 0; i < RB; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i], 16);
-    }
+    for (int i = 0; i < RB; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i], 16);
 #pragma unroll
-    for (int dd = (RB == 32 ? 16 : 8), n = RB; dd >= 1; dd >>= 1, n >>= 1) {
+    for (int dd = RB / 2, n = RB; dd >= 1; dd >>= 1, n >>= 1) {
       const bool up = (lane & dd) != 0;
 #pragma unroll
       for (int i = 0; i < n / 2; ++i) {

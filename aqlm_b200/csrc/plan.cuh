@@ -21,28 +21,16 @@ inline int env_int(const char* name, int dflt) {
 // Experiment switches (environment variables), read ONCE per process -- not per launch -- and again only when a tool
 // calls aqlm_b200_reload_tunables() after changing the environment.  Defaults are the shipped configuration.
 struct Tunables {
-  int pdl, gemv_ctas_per_sm, gemv_threads, gather_mode, gemv_v2, force_generic;
-  int disable_lut, lut_ctas_per_sm, lut_debug, lut_cluster, lut_batch_loop, lut_rb16, lut_c2_rb;
+  int pdl, gemv_ctas_per_sm, force_generic;
+  int disable_lut, lut_ctas_per_sm, lut_batch_loop;
   int disable_wgmma, gemm_stages, gemm_ksplit, gemm_gather_mode, gemm_tile_m;
   void load() {
     pdl = env_int("AQLM_B200_PDL", 1);
     gemv_ctas_per_sm = env_int("AQLM_B200_GEMV_CTAS_PER_SM", 1);
-    gemv_threads = env_int("AQLM_B200_GEMV_THREADS", kGemv1x16Threads);
-    gather_mode = env_int("AQLM_B200_GATHER_MODE", 0);
-    gemv_v2 = env_int("AQLM_B200_GEMV_V2", 1);
     force_generic = env_int("AQLM_B200_FORCE_GENERIC", 0);
     disable_lut = env_int("AQLM_B200_DISABLE_LUT", 0);
     lut_ctas_per_sm = env_int("AQLM_B200_LUT_CTAS_PER_SM", 2);  // 128 regs x 256 threads: registers allow 2
-    lut_debug = env_int("AQLM_B200_LUT_DEBUG", 0);
     lut_batch_loop = env_int("AQLM_B200_LUT_BATCH_LOOP", 1);  // batch 2-3 on 256-entry codebooks: one LUT launch per row
-    lut_rb16 = env_int("AQLM_B200_LUT_RB16", 0);  // cluster kernel: 16-row warp batches on 768 threads (experiment)
-    lut_c2_rb = env_int("AQLM_B200_LUT_C2_RB", 0);  // cluster kernel, second form: rows per warp batch (0: 16; 16; 32)
-    // K <= 2, in <= 4096: slab CTAs form a cluster, DSMEM reduction.  0: off (workspace kernel), 1: first form, 2: second form,
-    // 3 (default, automatic): the second form with 16-row warp batches at every row-block size.  Measured with
-    // tools/probe_lut2.py on an H100 80GB HBM3 (400 W limit): fastest or tied on every probed shape, e.g. 2x8 4096 -> 11008 /
-    // 12288 / 22016 in 12.1 / 12.6 / 17.9 us against 13.7 / 15.3 / 24.4 us for the first form and 14.4 / 17.1 / 26.9 us
-    // for 32-row batches.
-    lut_cluster = env_int("AQLM_B200_LUT_CLUSTER", 3);
     disable_wgmma = env_int("AQLM_B200_DISABLE_WGMMA", 0);
     gemm_stages = env_int("AQLM_B200_GEMM_STAGES", 0);
     gemm_ksplit = env_int("AQLM_B200_GEMM_KSPLIT", 0);
@@ -96,7 +84,7 @@ inline bool lut_cluster_eligible(const aqlm_b200_weight_t& w, const void* input,
   const int K = w.num_codebooks;
   const int in_groups = (int)(w.in_features / 8);
   if (batch != 1 || w.nbits_per_codebook != 8 || w.in_group_size != 8 || (K != 1 && K != 2)) return false;
-  if (!t.lut_cluster || t.disable_lut || t.lut_debug) return false;
+  if (t.disable_lut) return false;
   if ((in_groups & 1) || in_groups > 8 * kLutCJ) return false;
   return !((reinterpret_cast<uintptr_t>(w.codes) & 3) || (reinterpret_cast<uintptr_t>(input) & 3));
 }

@@ -492,6 +492,23 @@ def test_lut_gemv_kx8(K, fin, fout):
     assert torch.equal(y, y2)  # fixed-order slab reduction
 
 
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
+@pytest.mark.parametrize("bias", [True, False])
+@pytest.mark.parametrize("K", [1, 2])
+@pytest.mark.parametrize("fin,fout", [(4096, 4096), (4096, 12288), (4096, 22016), (1024, 200)])
+def test_lut_cluster_kernel(dtype, bias, K, fin, fout):
+    """The cluster LUT GEMV (K <= 2, in_features <= 4096; csrc/gemv_lut.cuh) on row blocks of 32 .. 1472 rows: one
+    round of warps and several, both the 768- and the 1024-thread build, all rows against the C oracle."""
+    from aqlm_b200.inference_kernels import cuda_kernel
+
+    t = gpu_case(fin, fout, K, 8, 1, dtype=dtype, seed=K * 77 + fin + fout, bias=bias)
+    y = cuda_kernel.matmat(t["x"], t["codes"], t["codebooks"], t["scales"], t["bias"])
+    rel = c_oracle_check(t, y)
+    assert rel < (TOL_FP16_TIGHT if dtype == torch.float16 else TOL_BF16), rel
+    y2 = cuda_kernel.matmat(t["x"], t["codes"], t["codebooks"], t["scales"], t["bias"])
+    assert torch.equal(y, y2)  # fixed-order cross-slab sum
+
+
 @pytest.mark.parametrize("K,batch", [(2, 2), (2, 5), (8, 3), (1, 6)])
 def test_kx8_small_batches_full_size(K, batch):
     """Batch 2-6 on 256-entry codebooks (the reference loops its matvec per row, cuda_kernel.cpp:387-421)."""

@@ -42,8 +42,7 @@ MAX_CLUSTERS = [-1, 1, 7, 16, 66, 132]
 # switch settings, each on a smaller grid of the plans it can change
 FORCED_GEMM = ([("GEMM_TILE_M", v) for v in (127, 65, 40, 8, 200)] + [("GEMM_KSPLIT", v) for v in (1, 3, 16, 999)]
                + [("GEMM_STAGES", v) for v in (2, 4, 5)] + [("DISABLE_WGMMA", 1)])
-FORCED_LUT = ([("DISABLE_LUT", 1), ("LUT_DEBUG", 1)] + [("LUT_CTAS_PER_SM", v) for v in (1, 3)]
-              + [("LUT_CLUSTER", v) for v in (0, 1, 3)])
+FORCED_LUT = [("DISABLE_LUT", 1)] + [("LUT_CTAS_PER_SM", v) for v in (1, 3)]
 FORCED_SHAPES = [(1152, 456), (4096, 4096), (8192, 28672)]
 FORCED_BATCHES = [1, 17, 300, 4096]
 

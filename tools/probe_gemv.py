@@ -1,7 +1,7 @@
 """Per-shape timing probe of the fused GEMV (and large-batch op): CUDA-graph replay over rotating weight copies
 (so codes come from HBM, not L2), CUDA events, reported as us and code-bytes GB/s vs the measured HBM peak.
 
-    python tools/probe_gemv.py [--schemes 1x16,2x8,8x8] [--batches 1,2,4,8] [--modes 0,1,2] [--out FILE]
+    python tools/probe_gemv.py [--schemes 1x16,2x8,8x8] [--batches 1,2,4,8] [--out FILE]
 """
 import argparse
 import json
@@ -61,7 +61,6 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--schemes", default="1x16,2x8,8x8")
     ap.add_argument("--batches", default="1")
-    ap.add_argument("--modes", default="0")
     ap.add_argument("--ctas", default="8")
     ap.add_argument("--op", default="matmat")
     ap.add_argument("--shapes", default="4096x4096,4096x1024,4096x14336,14336x4096,4096x11008,8192x8192,8192x28672")
@@ -80,21 +79,18 @@ def main():
             ws = make_weights(fin, fout, K, nbits, 8, copies, dev)
             for batch in (int(b) for b in args.batches.split(",")):
                 x = torch.randn((batch, fin), dtype=torch.float16, device=dev)
-                for mode in args.modes.split(","):
-                    for ctas in args.ctas.split(","):
-                        os.environ["AQLM_B200_GATHER_MODE"] = mode
-                        os.environ["AQLM_B200_GEMV_CTAS_PER_SM"] = ctas
-                        _cabi.reload_tunables()
-                        fns = [(lambda w=w: op(x, w[0], w[1], w[2], None)) for w in ws]
-                        us = time_graph(fns)
-                        gbs = cbytes / us / 1e3
-                        tflops = 2.0 * batch * fin * fout / us / 1e6
-                        row = dict(scheme=scheme, in_features=fin, out_features=fout, batch=batch, tflops=round(tflops, 1),
-                                   gather_mode=int(mode),
-                                   ctas_per_sm=int(ctas), op=args.op, us=round(us, 3), code_GBps=round(gbs, 1),
-                                   frac_of_hbm_peak=round(gbs / peak, 4), peak=peak_kind, rotating_copies=copies)
-                        rows.append(row)
-                        print(json.dumps(row), flush=True)
+                for ctas in args.ctas.split(","):
+                    os.environ["AQLM_B200_GEMV_CTAS_PER_SM"] = ctas
+                    _cabi.reload_tunables()
+                    fns = [(lambda w=w: op(x, w[0], w[1], w[2], None)) for w in ws]
+                    us = time_graph(fns)
+                    gbs = cbytes / us / 1e3
+                    tflops = 2.0 * batch * fin * fout / us / 1e6
+                    row = dict(scheme=scheme, in_features=fin, out_features=fout, batch=batch, tflops=round(tflops, 1),
+                               ctas_per_sm=int(ctas), op=args.op, us=round(us, 3), code_GBps=round(gbs, 1),
+                               frac_of_hbm_peak=round(gbs / peak, 4), peak=peak_kind, rotating_copies=copies)
+                    rows.append(row)
+                    print(json.dumps(row), flush=True)
             del ws
             torch.cuda.empty_cache()
     if args.out:

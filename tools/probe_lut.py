@@ -1,5 +1,5 @@
-"""Phase breakdown of the Kx8 LUT GEMV: time the kernel with phases switched off (AQLM_B200_LUT_DEBUG bits: 1 no lookups,
-2 no LUT build, 4 no partials/fix-up) -- CUDA-graph replay over rotating weight copies, CUDA events."""
+"""Batch-1 Kx8 LUT GEMV against its alternatives: the shipped plan, one LUT CTA per SM, the gather kernel (no LUT), and at
+batch 2 / 4 the gather kernel against one LUT launch per row -- CUDA-graph replay over rotating weight copies, CUDA events."""
 import json
 import os
 import sys
@@ -24,21 +24,13 @@ def main():
                torch.randn((K, 256, 1, 8), dtype=torch.float16, device=dev),
                (0.75 + 0.5 * torch.rand((fout, 1, 1, 1), device=dev)).half()) for _ in range(copies)]
         x = torch.randn((1, fin), dtype=torch.float16, device=dev)
-        for dbg, label in ((0, "full"), (1, "no lookups"), (2, "no LUT build"), (4, "no fix-up"), (5, "build only"), (6, "lookups only"),
-                           (7, "launch + prologue only")):
-            os.environ["AQLM_B200_LUT_DEBUG"] = str(dbg)
-            _cabi.reload_tunables()
-            us = timed([(lambda w=w: cuda_kernel.matmat(x, w[0], w[1], w[2], None)) for w in ws])
-            print(json.dumps(dict(scheme=f"{K}x8", shape=f"{fin}x{fout}", phase=label, us=round(us, 2),
-                                  code_GBps=round(cb / us / 1e3, 1))), flush=True)
-        os.environ["AQLM_B200_LUT_DEBUG"] = "0"
-        _cabi.reload_tunables()
-        # the ctas-per-SM knob and the plain gather kernel for comparison
-        for env, label in (({"AQLM_B200_LUT_CTAS_PER_SM": "1"}, "1 CTA/SM"), ({"AQLM_B200_DISABLE_LUT": "1"}, "gather kernel (no LUT)")):
+        # the shipped plan, the ctas-per-SM knob and the plain gather kernel
+        for env, label in (({}, "shipped"), ({"AQLM_B200_LUT_CTAS_PER_SM": "1"}, "1 CTA/SM"),
+                           ({"AQLM_B200_DISABLE_LUT": "1"}, "gather kernel (no LUT)")):
             os.environ.update(env)
             _cabi.reload_tunables()
             us = timed([(lambda w=w: cuda_kernel.matmat(x, w[0], w[1], w[2], None)) for w in ws])
-            print(json.dumps(dict(scheme=f"{K}x8", shape=f"{fin}x{fout}", phase=label, us=round(us, 2),
+            print(json.dumps(dict(scheme=f"{K}x8", shape=f"{fin}x{fout}", variant=label, us=round(us, 2),
                                   code_GBps=round(cb / us / 1e3, 1))), flush=True)
             for k in env:
                 os.environ.pop(k)
