@@ -87,6 +87,7 @@ def lib():
                 L.aqlm_b200_matmat_dequant_workspace_bytes.argtypes = [wp, i64]
                 L.aqlm_b200_matmat_dequant_workspace_bytes.restype = ctypes.c_size_t
                 L.aqlm_b200_matmat_dequant_ws.argtypes = [wp, vp, vp, i64, vp, ctypes.c_size_t, vp]
+                L.aqlm_b200_matmat_dequant_ex.argtypes = [wp, vp, vp, i64, u32, vp, ctypes.c_size_t, vp]
                 L.aqlm_b200_dequant.argtypes = [wp, vp, ctypes.c_int, vp]
                 L.aqlm_b200_matmat_dequant_transposed.argtypes = [wp, vp, vp, i64, vp, ctypes.c_size_t, vp]
                 L.aqlm_b200_matmat_dequant_transposed_workspace_bytes.argtypes = [wp, i64]

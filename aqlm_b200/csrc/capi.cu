@@ -484,8 +484,8 @@ template <typename T>
 constexpr CUtensorMapDataType kTmapType = DT<T>::is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
 
 template <typename T, int K, int CB>
-static int launch_gemm(const aqlm_b200_weight_t* w, const void* input, void* output, int64_t batch, const GemmPlan& g,
-                       void* workspace, const DeviceInfo* di, cudaStream_t st) {
+static int launch_gemm(const aqlm_b200_weight_t* w, const void* input, void* output, int64_t batch, bool partial,
+                       const GemmPlan& g, void* workspace, const DeviceInfo* di, cudaStream_t st) {
   const size_t row_bytes = (size_t)(w->in_features / 8) * K * CB;
   CUtensorMap tx, tc;
   if (int rc = encode_tmap(&tx, "x", kTmapType<T>, input, w->in_features, batch, w->in_features * 2, kGemmBlockK,
@@ -496,8 +496,9 @@ static int launch_gemm(const aqlm_b200_weight_t* w, const void* input, void* out
     return rc;
   GemmParams p;
   p.codebooks = w->codebooks;
-  p.scales = w->scales;
-  p.bias = w->bias;
+  p.scales = partial ? nullptr : w->scales;
+  p.bias = partial ? nullptr : w->bias;
+  p.partial_f32 = partial ? 1 : 0;
   p.y = output;
   p.ws_counters = g.ksplit > 1 ? reinterpret_cast<unsigned int*>(workspace) : nullptr;
   p.ws_partials = g.ksplit > 1 ? reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + g.counters_bytes) : nullptr;
@@ -688,7 +689,7 @@ int aqlm_b200_matmat(const aqlm_b200_weight_t* w, const void* input, void* outpu
 }
 
 size_t aqlm_b200_matmat_dequant_workspace_bytes(const aqlm_b200_weight_t* w, int64_t batch) {
-  if (validate(w, true) != AQLM_B200_OK || batch <= 0) return 0;
+  if (validate(w, false) != AQLM_B200_OK || batch <= 0) return 0;  // the plan never reads scales
   const DeviceInfo* di = device_info();
   if (!di) return 0;
   const GemmPlan g = gemm_plan(*w, batch, *di, tun(), true);
@@ -696,9 +697,10 @@ size_t aqlm_b200_matmat_dequant_workspace_bytes(const aqlm_b200_weight_t* w, int
   return g.counters_bytes + g.partials_bytes;
 }
 
-int aqlm_b200_matmat_dequant_ws(const aqlm_b200_weight_t* w, const void* input, void* output, int64_t batch,
-                                void* workspace, size_t workspace_bytes, void* stream) {
-  int rc = validate(w, true);
+int aqlm_b200_matmat_dequant_ex(const aqlm_b200_weight_t* w, const void* input, void* output, int64_t batch,
+                                uint32_t flags, void* workspace, size_t workspace_bytes, void* stream) {
+  const bool partial = (flags & AQLM_B200_FLAG_PARTIAL_F32) != 0;
+  int rc = validate(w, !partial);
   if (rc) return rc;
   if (batch < 0) return fail(AQLM_B200_ERR_SHAPE, "negative batch");
   if (batch == 0) return AQLM_B200_OK;
@@ -711,13 +713,18 @@ int aqlm_b200_matmat_dequant_ws(const aqlm_b200_weight_t* w, const void* input, 
   if (!g.ok || (reinterpret_cast<uintptr_t>(input) & 15) != 0) {
     // shapes the tensor-core kernel does not cover (in_group 16, in_features % 64 != 0, odd KxN):
     // batch passes of 8 rows through the fused gather+dequant+dot kernel
-    return aqlm_b200_matmat_ex(w, input, output, batch, 0, stream);
+    return aqlm_b200_matmat_ex(w, input, output, batch, flags, stream);
   }
   return with_dtype(w->dtype, [&](auto tag) {
     return with_gemm_scheme(w, [&](auto K, auto CB) {
-      return launch_gemm<typename decltype(tag)::type, K, CB>(w, input, output, batch, g, workspace, di, st);
+      return launch_gemm<typename decltype(tag)::type, K, CB>(w, input, output, batch, partial, g, workspace, di, st);
     });
   });
+}
+
+int aqlm_b200_matmat_dequant_ws(const aqlm_b200_weight_t* w, const void* input, void* output, int64_t batch,
+                                void* workspace, size_t workspace_bytes, void* stream) {
+  return aqlm_b200_matmat_dequant_ex(w, input, output, batch, 0, workspace, workspace_bytes, stream);
 }
 
 int aqlm_b200_matmat_dequant(const aqlm_b200_weight_t* w, const void* input, void* output, int64_t batch,
@@ -859,31 +866,41 @@ int aqlm_b200_allreduce_scale_bias(aqlm_b200_comm* c, const float* partial, cons
                                    void* output, int64_t batch, int64_t out_features, int32_t dtype, void* stream) {
   if (!c || !partial || !scales || !output) return fail(AQLM_B200_ERR_SHAPE, "NULL pointer");
   if (dtype != AQLM_B200_F16 && dtype != AQLM_B200_BF16) return fail(AQLM_B200_ERR_DTYPE, "dtype must be f16/bf16");
-  const int64_t n = batch * out_features;
-  if (n <= 0) return AQLM_B200_OK;
-  if (n > c->max_elems || (out_features & 3)) return fail(AQLM_B200_ERR_SHAPE, "allreduce: %lld elements exceed the communicator's %lld (or out_features %% 4 != 0)", (long long)n, c->max_elems);
+  if (batch <= 0 || out_features <= 0) return AQLM_B200_OK;
+  if (out_features > c->max_elems || (out_features & 3))
+    return fail(AQLM_B200_ERR_SHAPE, "allreduce: out_features %lld exceeds the communicator's %lld elements (or %% 4 != 0)",
+                (long long)out_features, c->max_elems);
   const DeviceInfo* di;
   if (int rc = current_device(&di)) return rc;
   PeerParams p;
   for (int r = 0; r < kPeerMaxWorld; ++r) p.peer_base[r] = r < c->world ? c->peer_base[r] : nullptr;
-  p.local = partial;
   p.scales = scales;
   p.bias = bias;
-  p.y = output;
   p.step = c->local_state;
   p.tickets = c->local_state + 1;
   p.max_elems = c->max_elems;
-  p.n = (int)n;
   p.out_features = (int)out_features;
   p.rank = c->rank;
   p.world = c->world;
-  int grid = (int)((n / 4 + kPeerThreads - 1) / kPeerThreads);
-  if (grid > kPeerMaxCtas) grid = kPeerMaxCtas;  // one flag per (source rank, CTA slice); every rank derives the same grid from n
-  if (grid < 1) grid = 1;
-  return with_dtype(dtype, [&](auto tag) {
-    return launch<peer_allreduce_epilogue_kernel<typename decltype(tag)::type>>(
-        di, grid, kPeerThreads, 0, reinterpret_cast<cudaStream_t>(stream), 0, p);
-  });
+  // A call larger than the communicator's slots runs as consecutive exchanges of whole rows, each one launch on a row
+  // slice of `partial` and `output`.  Every rank derives the same chunking from max_elems (checked equal at
+  // construction), so all ranks run the same number of steps.
+  const int64_t chunk_rows = c->max_elems / out_features;
+  for (int64_t b0 = 0; b0 < batch; b0 += chunk_rows) {
+    const int64_t n = (batch - b0 < chunk_rows ? batch - b0 : chunk_rows) * out_features;
+    p.local = partial + b0 * out_features;
+    p.y = reinterpret_cast<uint8_t*>(output) + (size_t)(b0 * out_features) * 2;
+    p.n = (int)n;
+    int grid = (int)((n / 4 + kPeerThreads - 1) / kPeerThreads);
+    if (grid > kPeerMaxCtas) grid = kPeerMaxCtas;  // one flag per (source rank, CTA slice); every rank derives the same grid from n
+    if (grid < 1) grid = 1;
+    const int rc = with_dtype(dtype, [&](auto tag) {
+      return launch<peer_allreduce_epilogue_kernel<typename decltype(tag)::type>>(
+          di, grid, kPeerThreads, 0, reinterpret_cast<cudaStream_t>(stream), 0, p);
+    });
+    if (rc) return rc;
+  }
+  return AQLM_B200_OK;
 }
 
 int aqlm_b200_matmat_allreduce(aqlm_b200_comm* c, const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg,

@@ -10,7 +10,8 @@
 //   B = the activation tile X[n0:n0+N, k0:k0+64], TMA-loaded (OOB rows zero-filled, so any batch works);
 //   two consumer warpgroups (rows 0-63 and 64-127 of the tile) issue wgmma.mma_async (64 x N x 16, fp16 or bf16
 //   operands, fp32 accumulate in registers), release the smem stage through an mbarrier once their wgmma group has
-//   completed, and apply scale + bias in the epilogue.
+//   completed, and apply scale + bias in the epilogue (or, with partial_f32, store the unscaled fp32 sums that an
+//   in_features-sharded linear all-reduces).
 // Warp roles: warps 0-7 consumers, warp 8 TMA (X tiles and code tiles), warps 9-16 dequant producers.
 // Grid = (M tiles, K splits, N tiles).  The kernel is bound by the per-SM codebook-gather rate, so the K dimension is
 // split to put every SM to work; split partials go through an fp32 workspace and the LAST-arriving CTA of each tile
@@ -18,6 +19,8 @@
 #pragma once
 
 #include <cuda.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -50,6 +53,7 @@ struct GemmParams {
   int stages;
   int tile_m;           // output rows per CTA tile (<= 128): ragged tile heights balance the grid
   int gather_mode;      // 0: ld.global.nc (L1 allocate), 1: ld.global.cg
+  int partial_f32;      // 1: y is fp32 and gets the UNSCALED sums (no scale, no bias; scales / bias may be null)
 };
 
 // ---- PTX wrappers -----------------------------------------------------------------------------------
@@ -227,11 +231,11 @@ __host__ __device__ inline GemmSmem gemm_smem_layout(int stages, int n_tile) {
 
 // Split-K fix-up shared by both GEMM kernels: the LAST-arriving split of a tile adds all partials in split order
 // (deterministic) with the whole CTA; partials are [split][column][128 rows].  Writes y[n * ld + row0 + r] =
-// v * scale[row] + bias[row] (scales == nullptr: no scale / bias).
-template <typename T>
+// v * scale[row] + bias[row] (scales == nullptr: no scale / bias); an fp32 output (OutT = float) gets the sum v itself.
+template <typename T, typename OutT = T>
 __device__ __forceinline__ void gemm_splitk_fixup(uint32_t* flag, unsigned int* counter, const float* parts, int ksplit, int N,
-                                                  int ncols, T* y, long long ld, int n0, int row0, int rows, const T* scales,
-                                                  const T* bias) {
+                                                  int ncols, OutT* y, long long ld, int n0, int row0, int rows,
+                                                  const T* scales, const T* bias) {
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -262,7 +266,9 @@ __device__ __forceinline__ void gemm_splitk_fixup(uint32_t* flag, unsigned int* 
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
           const int cc = c + u * kPhases;
-          if (cc < ncols) y[(size_t)(n0 + cc) * ld + row] = DT<T>::from_float(fmaf(v[u], sc, bi));
+          if (cc >= ncols) continue;
+          if constexpr (std::is_same<OutT, float>::value) y[(size_t)(n0 + cc) * ld + row] = v[u];
+          else y[(size_t)(n0 + cc) * ld + row] = DT<T>::from_float(fmaf(v[u], sc, bi));
         }
       }
     }
@@ -360,7 +366,7 @@ gemm_dequant_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_con
       const int row = m0 + row_in_tile;
       const bool row_ok = row_in_tile < TM && row < p.out_features;
       float sc = 1.f, bi = 0.f;
-      if (row_ok && p.ksplit == 1) {
+      if (row_ok && p.ksplit == 1 && !p.partial_f32) {
         sc = DT<T>::to_float(reinterpret_cast<const T*>(p.scales)[row]);
         if (p.bias) bi = DT<T>::to_float(reinterpret_cast<const T*>(p.bias)[row]);
       }
@@ -371,7 +377,11 @@ gemm_dequant_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_con
           const int col = 8 * i + 2 * (lane & 3) + c;
           const float v = acc[4 * i + 2 * j + c];
           if (p.ksplit == 1) {
-            if (row_ok && n0 + col < p.batch) y[(size_t)(n0 + col) * p.out_features + row] = DT<T>::from_float(fmaf(v, sc, bi));
+            if (row_ok && n0 + col < p.batch) {
+              const size_t o = (size_t)(n0 + col) * p.out_features + row;
+              if (p.partial_f32) reinterpret_cast<float*>(p.y)[o] = v;
+              else y[o] = DT<T>::from_float(fmaf(v, sc, bi));
+            }
           } else {
             my_part[(size_t)col * kGemmBlockM + row_in_tile] = v;
           }
@@ -522,10 +532,15 @@ gemm_dequant_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_con
 
   if (p.ksplit > 1) {
     griddep_wait();
-    gemm_splitk_fixup<T>(reinterpret_cast<uint32_t*>(gbase + L.flag), p.ws_counters + tile_id,
-                         p.ws_partials + (tile_id * p.ksplit) * (size_t)N * kGemmBlockM, p.ksplit, N,
-                         min(N, p.batch - n0), y, p.out_features, n0, m0, min(TM, p.out_features - m0),
-                         reinterpret_cast<const T*>(p.scales), reinterpret_cast<const T*>(p.bias));
+    uint32_t* flag = reinterpret_cast<uint32_t*>(gbase + L.flag);
+    const float* parts = p.ws_partials + (tile_id * p.ksplit) * (size_t)N * kGemmBlockM;
+    const int ncols = min(N, p.batch - n0), rows = min(TM, p.out_features - m0);
+    if (p.partial_f32)
+      gemm_splitk_fixup<T, float>(flag, p.ws_counters + tile_id, parts, p.ksplit, N, ncols, reinterpret_cast<float*>(p.y),
+                                  p.out_features, n0, m0, rows, nullptr, nullptr);
+    else
+      gemm_splitk_fixup<T>(flag, p.ws_counters + tile_id, parts, p.ksplit, N, ncols, y, p.out_features, n0, m0, rows,
+                           reinterpret_cast<const T*>(p.scales), reinterpret_cast<const T*>(p.bias));
   }
 }
 

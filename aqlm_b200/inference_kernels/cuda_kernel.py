@@ -160,6 +160,17 @@ def _call_matmat_ws(device, w, flat_input, flat_output, flags: int) -> None:
                                           ws.numel() if ws is not None else 0, _stream_ptr(device)))
 
 
+def _call_matmat_dequant_ex(device, w, flat_input, flat_output, flags: int) -> None:
+    batch = flat_input.shape[0]
+    with _on_device(device):
+        L = _cabi.lib()
+        need = L.aqlm_b200_matmat_dequant_workspace_bytes(ctypes.byref(w), batch) if batch > 0 else 0
+        ws = _workspace(device, need) if need else None
+        _cabi.check(L.aqlm_b200_matmat_dequant_ex(ctypes.byref(w), flat_input.data_ptr(), flat_output.data_ptr(), batch,
+                                                  flags, ws.data_ptr() if ws is not None else None,
+                                                  ws.numel() if ws is not None else 0, _stream_ptr(device)))
+
+
 def matmat(input, codes, codebooks, scales, bias=None) -> torch.Tensor:
     """Fused gather + additive dequant + GEMV (+scale+bias), any scheme; for small batch (reference `*_matmat`).
     Batch-1 calls on 256-entry codebooks run the dot-product-LUT kernel."""
@@ -172,15 +183,8 @@ def matmat(input, codes, codebooks, scales, bias=None) -> torch.Tensor:
 def matmat_dequant(input, codes, codebooks, scales, bias=None) -> torch.Tensor:
     """Fused dequant + wgmma tensor-core GEMM (+scale+bias); for large batch (reference `*_matmat_dequant`)."""
     device, w, flat_input = _prepare(input, codes, codebooks, scales, bias)
-    batch = flat_input.shape[0]
-    flat_output = torch.empty((batch, w.out_features), dtype=input.dtype, device=device)
-    with _on_device(device):
-        L = _cabi.lib()
-        need = L.aqlm_b200_matmat_dequant_workspace_bytes(ctypes.byref(w), batch) if batch > 0 else 0
-        ws = _workspace(device, need) if need else None
-        _cabi.check(L.aqlm_b200_matmat_dequant_ws(ctypes.byref(w), flat_input.data_ptr(), flat_output.data_ptr(), batch,
-                                                  ws.data_ptr() if ws is not None else None,
-                                                  ws.numel() if ws is not None else 0, _stream_ptr(device)))
+    flat_output = torch.empty((flat_input.shape[0], w.out_features), dtype=input.dtype, device=device)
+    _call_matmat_dequant_ex(device, w, flat_input, flat_output, 0)
     return flat_output.reshape(input.shape[:-1] + (w.out_features,))
 
 
@@ -210,12 +214,16 @@ def matmat_grouped(input, codes, codebooks_stacked, scales, bias, seg_rows, part
 
 
 def matmat_partial(input, codes, codebooks) -> torch.Tensor:
-    """UNSCALED fp32 partial products [batch, out] of an in_features shard (to be all-reduced)."""
+    """UNSCALED fp32 partial products [batch, out] of an in_features shard (to be all-reduced).  Above GEMV_MAX_ROWS
+    rows (prefill) this is the wgmma GEMM, as in QuantizedLinear; below, the GEMV / LUT kernels."""
+    from ..inference import GEMV_MAX_ROWS
+
     device = _require_cuda(input, codes, codebooks)
     w = make_weight(codes, codebooks, None, None)
     flat_input = input.reshape(-1, input.shape[-1]).contiguous()
     out = torch.empty((flat_input.shape[0], w.out_features), dtype=torch.float32, device=device)
-    _call_matmat_ws(device, w, flat_input, out, _cabi.FLAG_PARTIAL_F32)
+    call = _call_matmat_dequant_ex if flat_input.shape[0] > GEMV_MAX_ROWS else _call_matmat_ws
+    call(device, w, flat_input, out, _cabi.FLAG_PARTIAL_F32)
     return out
 
 

@@ -3,7 +3,9 @@
 `PeerComm.allreduce_scale_bias(partial, scales, bias, dtype)` is the fused replacement for
 `dist.all_reduce(partial); scale_bias(partial)`: ONE kernel pushes the fp32 partials into every peer's buffer,
 publishes a release flag, waits for all ranks' flags, adds the W partial vectors in rank order and applies scale + bias
-(`csrc/peer_allreduce.cuh`).  `torch.distributed` is used only once, at construction, to exchange the 64-byte IPC handles.
+(`csrc/peer_allreduce.cuh`).  A batch larger than the communicator's `max_elems` runs as consecutive exchanges of whole
+rows.  `torch.distributed` is used only at construction, to check that every rank has the same `max_elems` and to
+exchange the 64-byte IPC handles.
 """
 from __future__ import annotations
 
@@ -17,6 +19,13 @@ from . import _cabi
 from .inference_kernels.cuda_kernel import _DTYPES, _on_device, _require_cuda, _stream_ptr, make_weight
 
 
+def check_same_max_elems(sizes) -> None:
+    """Raise ValueError unless every rank's communicator has the same max_elems (`sizes[r]` is rank r's)."""
+    if len(set(sizes)) > 1:
+        raise ValueError("PeerComm: every rank must pass the same max_elems; got "
+                         + ", ".join(f"rank {r}: {v}" for r, v in enumerate(sizes)))
+
+
 class PeerComm:
     def __init__(self, group=None, max_elems: int = 8 * 28672, device: Optional[torch.device] = None):
         self.group = group
@@ -24,6 +33,12 @@ class PeerComm:
         self.world = dist.get_world_size(group)
         self.device = device or torch.device("cuda", torch.cuda.current_device())
         self.max_elems = (int(max_elems) + 3) // 4 * 4
+        # An exchange larger than max_elems runs in chunks of max_elems // out_features rows: ranks with different
+        # max_elems would run different numbers of steps and wait for each other forever.  Checked before anything is
+        # allocated, and every rank sees the same gathered list, so either all ranks raise or none does.
+        sizes = [None] * self.world
+        dist.all_gather_object(sizes, self.max_elems, group=group)
+        check_same_max_elems(sizes)
         L = _cabi.lib()
         with torch.cuda.device(self.device):
             nbytes = L.aqlm_b200_comm_shared_bytes(self.world, self.max_elems)

@@ -41,7 +41,7 @@ typedef enum {
 
 typedef enum { AQLM_B200_F16 = 0, AQLM_B200_BF16 = 1 } aqlm_b200_dtype;
 
-/* flags for aqlm_b200_matmat_ex */
+/* flags for aqlm_b200_matmat_ex, aqlm_b200_matmat_ws and aqlm_b200_matmat_dequant_ex */
 #define AQLM_B200_FLAG_PARTIAL_F32 1u /* write UNSCALED fp32 partial sums (no scale, no bias): the per-rank
                                           result of an in_features-sharded matvec, to be all-reduced */
 
@@ -100,10 +100,18 @@ int aqlm_b200_matmat_dequant(const aqlm_b200_weight_t* w, const void* input, voi
 /* Same with a caller-owned workspace, which lets the kernel split the K dimension across otherwise idle SMs
  * (the reduction is deterministic).  The first aqlm_b200_matmat_dequant_workspace_bytes() bytes... the whole
  * workspace must be ZERO before the first use and is left zero-initialised where it matters (tile counters),
- * so one persistent buffer per stream can be reused without memsets. */
+ * so one persistent buffer per stream can be reused without memsets.  The size depends on the shape, the scheme and the
+ * batch only: w->scales may be NULL here (as for a call with AQLM_B200_FLAG_PARTIAL_F32). */
 size_t aqlm_b200_matmat_dequant_workspace_bytes(const aqlm_b200_weight_t* w, int64_t batch);
 int aqlm_b200_matmat_dequant_ws(const aqlm_b200_weight_t* w, const void* input, void* output, int64_t batch,
                                 void* workspace, size_t workspace_bytes, void* stream);
+/* Same with flags.  AQLM_B200_FLAG_PARTIAL_F32: `output` is fp32 [batch, out_features] and receives the UNSCALED sums
+ * (scales and bias may be NULL and are ignored), as from aqlm_b200_matmat_ex -- the large-batch (prefill) form of an
+ * in_features-sharded linear's partial product.  Layouts the tensor-core kernel does not cover (in_group_size 16,
+ * in_features % 64 != 0, other KxN, an input that is not 16-byte aligned) run as aqlm_b200_matmat_ex with the same
+ * flags.  aqlm_b200_matmat_dequant_ws is this call with flags = 0. */
+int aqlm_b200_matmat_dequant_ex(const aqlm_b200_weight_t* w, const void* input, void* output, int64_t batch,
+                                uint32_t flags, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Materialise W [out_features, in_features] (x scales when apply_scales != 0).  Replaces
  * code{1x16,2x8,1x8}_dequant (cuda_kernel.cpp:184-227, 423-448, 588-613). */
@@ -131,7 +139,10 @@ int aqlm_b200_scale_bias(const float* partial, const void* scales, const void* b
  * from the W mapped pointers (peer_ptrs[rank] = its own buffer).  aqlm_b200_allreduce_scale_bias then does, in ONE
  * kernel: push my fp32 partials into every peer's buffer (P2P stores), publish a release flag, wait for all W flags,
  * add the W partials in rank order, apply scale + bias, write `output`.  Every rank must call it the same number of
- * times in the same order.  max_elems bounds batch*out_features of any call. */
+ * times in the same order, and every rank's communicator must have the same max_elems.  A call with
+ * batch*out_features > max_elems runs as consecutive exchanges of max_elems / out_features whole rows each (one kernel
+ * launch apiece); out_features itself must not exceed max_elems.  For aqlm_b200_matmat_allreduce below, max_elems
+ * bounds batch*out_features of any call. */
 typedef struct aqlm_b200_comm aqlm_b200_comm;
 size_t aqlm_b200_comm_shared_bytes(int world, int64_t max_elems);
 int aqlm_b200_shared_alloc(size_t bytes, void** ptr, void* handle64);
