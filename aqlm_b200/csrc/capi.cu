@@ -483,26 +483,34 @@ static int encode_tmap(CUtensorMap* map, const char* what, CUtensorMapDataType t
 template <typename T>
 constexpr CUtensorMapDataType kTmapType = DT<T>::is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
 
-template <typename T, int K, int CB>
-static int launch_gemm(const aqlm_b200_weight_t* w, const void* input, void* output, int64_t batch, bool partial,
-                       const GemmPlan& g, void* workspace, const DeviceInfo* di, cudaStream_t st) {
+// One launch of either GEMM.  Forward: b = x [batch][in_features], y [batch][out_features] (fp32 sums with `partial`).
+// TRANSPOSED (backward w.r.t. the input): b = grad_output [batch][out_features], y = grad_input [batch][in_features].
+// The directions differ in the code-tile map and in which side of W is the contraction; the rest is shared.
+template <typename T, int K, int CB, bool TRANSPOSED>
+static int launch_gemm(const aqlm_b200_weight_t* w, const void* b, void* y, int64_t batch, bool partial, const GemmPlan& g,
+                       void* workspace, const DeviceInfo* di, cudaStream_t st) {
+  using Dir = std::conditional_t<TRANSPOSED, GemmTransposed<K, CB>, GemmForward<K, CB>>;
+  const int64_t k_size = TRANSPOSED ? w->out_features : w->in_features;
   const size_t row_bytes = (size_t)(w->in_features / 8) * K * CB;
-  CUtensorMap tx, tc;
-  if (int rc = encode_tmap(&tx, "x", kTmapType<T>, input, w->in_features, batch, w->in_features * 2, kGemmBlockK,
+  CUtensorMap tb, tc;
+  if (int rc = encode_tmap(&tb, TRANSPOSED ? "grad_output" : "x", kTmapType<T>, b, k_size, batch, k_size * 2, kGemmBlockK,
                            g.n_tile, CU_TENSOR_MAP_SWIZZLE_128B))
     return rc;
-  if (int rc = encode_tmap(&tc, "codes", CU_TENSOR_MAP_DATA_TYPE_UINT8, w->codes, row_bytes, w->out_features, row_bytes,
-                           kCodeTileBytes, g.tile_m, CU_TENSOR_MAP_SWIZZLE_128B))
+  if (int rc = TRANSPOSED ? encode_tmap(&tc, "codes, transposed", CU_TENSOR_MAP_DATA_TYPE_UINT8, w->codes, row_bytes,
+                                        w->out_features, row_bytes, 16 * K * CB, kGemmTCtileRows, CU_TENSOR_MAP_SWIZZLE_NONE)
+                          : encode_tmap(&tc, "codes", CU_TENSOR_MAP_DATA_TYPE_UINT8, w->codes, row_bytes, w->out_features,
+                                        row_bytes, kCodeTileBytes, g.tile_m, CU_TENSOR_MAP_SWIZZLE_128B))
     return rc;
   GemmParams p;
   p.codebooks = w->codebooks;
   p.scales = partial ? nullptr : w->scales;
-  p.bias = partial ? nullptr : w->bias;
+  p.bias = partial || TRANSPOSED ? nullptr : w->bias;
   p.partial_f32 = partial ? 1 : 0;
-  p.y = output;
+  p.y = y;
   p.ws_counters = g.ksplit > 1 ? reinterpret_cast<unsigned int*>(workspace) : nullptr;
   p.ws_partials = g.ksplit > 1 ? reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + g.counters_bytes) : nullptr;
-  p.out_features = (int)w->out_features;
+  p.m_size = (int)(TRANSPOSED ? w->in_features : w->out_features);
+  p.k_size = (int)k_size;
   p.batch = (int)batch;
   p.nbits = w->nbits_per_codebook;
   p.total_kblocks = g.total_kblocks;
@@ -511,41 +519,9 @@ static int launch_gemm(const aqlm_b200_weight_t* w, const void* input, void* out
   p.tile_m = g.tile_m;
   p.gather_mode = tun().gemm_gather_mode >= 0 ? tun().gemm_gather_mode : (w->nbits_per_codebook > 8 ? 1 : 0);
   return with_n_tile(g.n_tile, [&](auto N) {
-    return launch<gemm_dequant_kernel<T, K, CB, N>>(di, dim3(g.m_tiles, g.ksplit, g.n_tiles), kGemmThreads,
-                                                    gemm_smem_layout(g.stages, N).total, st, 0, tx, tc, p);
-  });
-}
-
-// ---- fused dequant + TRANSPOSED wgmma GEMM (backward w.r.t. the input): host side ---------------------
-template <typename T, int K, int CB>
-static int launch_gemm_t(const aqlm_b200_weight_t* w, const void* grad_output, void* grad_input, int64_t batch,
-                         const GemmPlan& g, void* workspace, const DeviceInfo* di, cudaStream_t st) {
-  constexpr int GBT = 16 * K * CB;
-  const size_t row_bytes = (size_t)(w->in_features / 8) * K * CB;
-  CUtensorMap tg, tc;
-  if (int rc = encode_tmap(&tg, "grad_output", kTmapType<T>, grad_output, w->out_features, batch, w->out_features * 2,
-                           kGemmBlockK, g.n_tile, CU_TENSOR_MAP_SWIZZLE_128B))
-    return rc;
-  if (int rc = encode_tmap(&tc, "codes, transposed", CU_TENSOR_MAP_DATA_TYPE_UINT8, w->codes, row_bytes,
-                           w->out_features, row_bytes, GBT, kGemmTCtileRows, CU_TENSOR_MAP_SWIZZLE_NONE))
-    return rc;
-  GemmTParams p;
-  p.codebooks = w->codebooks;
-  p.scales = w->scales;
-  p.y = grad_input;
-  p.ws_counters = g.ksplit > 1 ? reinterpret_cast<unsigned int*>(workspace) : nullptr;
-  p.ws_partials = g.ksplit > 1 ? reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + g.counters_bytes) : nullptr;
-  p.in_features = (int)w->in_features;
-  p.out_features = (int)w->out_features;
-  p.batch = (int)batch;
-  p.nbits = w->nbits_per_codebook;
-  p.total_kblocks = g.total_kblocks;
-  p.ksplit = g.ksplit;
-  p.stages = g.stages;
-  p.gather_mode = tun().gemm_gather_mode >= 0 ? tun().gemm_gather_mode : (w->nbits_per_codebook > 8 ? 1 : 0);
-  return with_n_tile(g.n_tile, [&](auto N) {
-    return launch<gemm_dequant_t_kernel<T, K, CB, N>>(di, dim3(g.m_tiles, g.ksplit, g.n_tiles), kGemmThreads,
-                                                      gemm_t_smem_layout(g.stages, N, GBT).total, st, 0, tg, tc, p);
+    constexpr auto kernel = TRANSPOSED ? gemm_dequant_t_kernel<T, K, CB, N> : gemm_dequant_kernel<T, K, CB, N>;
+    return launch<kernel>(di, dim3(g.m_tiles, g.ksplit, g.n_tiles), kGemmThreads,
+                          gemm_smem_layout(g.stages, N, Dir::kCtileBytes).total, st, 0, tb, tc, p);
   });
 }
 
@@ -717,7 +693,7 @@ int aqlm_b200_matmat_dequant_ex(const aqlm_b200_weight_t* w, const void* input, 
   }
   return with_dtype(w->dtype, [&](auto tag) {
     return with_gemm_scheme(w, [&](auto K, auto CB) {
-      return launch_gemm<typename decltype(tag)::type, K, CB>(w, input, output, batch, partial, g, workspace, di, st);
+      return launch_gemm<typename decltype(tag)::type, K, CB, false>(w, input, output, batch, partial, g, workspace, di, st);
     });
   });
 }
@@ -774,7 +750,7 @@ int aqlm_b200_matmat_dequant_transposed(const aqlm_b200_weight_t* w, const void*
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   return with_dtype(w->dtype, [&](auto tag) {
     return with_gemm_scheme(w, [&](auto K, auto CB) {
-      return launch_gemm_t<typename decltype(tag)::type, K, CB>(w, grad_output, grad_input, batch, g, workspace, di, st);
+      return launch_gemm<typename decltype(tag)::type, K, CB, true>(w, grad_output, grad_input, batch, false, g, workspace, di, st);
     });
   });
 }

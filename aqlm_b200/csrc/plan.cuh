@@ -212,8 +212,8 @@ inline GemmPlan gemm_plan(const aqlm_b200_weight_t& w, int64_t batch, const Devi
   if (!gemm_scheme_ok(w, t) || 8 * K * cb > kCodeTileBytes || w.in_features % kGemmBlockK != 0) return g;
   g.total_kblocks = (int)(w.in_features / kGemmBlockK);
   gemm_n_tiles(batch, &g.n_tile, &g.n_tiles);
-  g.stages = gemm_stages([&](int s) { return gemm_smem_layout(s, g.n_tile).total; }, (size_t)di.max_smem_optin,
-                         t.gemm_stages, 4);
+  g.stages = gemm_stages([&](int s) { return gemm_smem_layout(s, g.n_tile, kGemmBlockM * kCodeTileBytes).total; },
+                         (size_t)di.max_smem_optin, t.gemm_stages, 4);
   if (!g.stages) return g;
   int best_tm = kGemmBlockM, best_ks = 1;
   double best = 1e30;
@@ -242,9 +242,9 @@ inline GemmPlan gemm_t_plan(const aqlm_b200_weight_t& w, int64_t batch, const De
   g.total_kblocks = (int)((w.out_features + kGemmBlockK - 1) / kGemmBlockK);
   g.m_tiles = (int)((w.in_features + kGemmBlockM - 1) / kGemmBlockM);
   gemm_n_tiles(batch, &g.n_tile, &g.n_tiles);
-  const int ctile_row_bytes = 16 * K * cb;
+  const int ctile_bytes = kGemmTCtileRows * 16 * K * cb;
   // forced stages: 2..3, i.e. never more than the unforced choice
-  g.stages = gemm_stages([&](int s) { return gemm_t_smem_layout(s, g.n_tile, ctile_row_bytes).total; },
+  g.stages = gemm_stages([&](int s) { return gemm_smem_layout(s, g.n_tile, ctile_bytes).total; },
                          (size_t)di.max_smem_optin, t.gemm_stages, 3);
   if (!g.stages) return g;
   if ((size_t)g.m_tiles * g.n_tiles > (size_t)kGemmMaxTiles) return g;

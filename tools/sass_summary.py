@@ -1,7 +1,7 @@
 """Opcode histogram per kernel of the shipped library (cuobjdump -sass), written as a small markdown table: the evidence
 that the wgmma / TMA paths are what the .so contains (HGMMA = wgmma.mma_async, UTMALDG = TMA tensor load, SYNCS = mbarrier,
 HMMA = mma.sync).  Runs on CPU (no GPU needed).
-    python tools/sass_summary.py > sass_summary.md"""
+    python tools/sass_summary.py [other/libaqlm_b200.so] > sass_summary.md"""
 import collections
 import os
 import re
@@ -15,7 +15,8 @@ KEY = ["HGMMA", "UTMALDG", "UTMAPF", "SYNCS", "HMMA", "LDG", "LDS", "STS", "LDGS
 
 
 def main():
-    sass = subprocess.run(["cuobjdump", "-sass", LIB], capture_output=True, text=True, check=True).stdout
+    lib = sys.argv[1] if len(sys.argv) > 1 else LIB
+    sass = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
     demangle = {}
     kernels = collections.OrderedDict()
     cur = None
@@ -40,7 +41,7 @@ def main():
         short = re.sub(r"^void aqlm_b200::", "", d)
         short = re.sub(r"\(.*$", "", short)
         agg[short] = c
-    print("# SASS opcode summary of aqlm_b200/csrc/libaqlm_b200.so (sm_90a)\n")
+    print(f"# SASS opcode summary of {os.path.relpath(lib, REPO)} (sm_90a)\n")
     print("`python tools/sass_summary.py` (cuobjdump -sass; counts are static instruction counts per kernel instantiation).\n")
     total = collections.Counter()
     for c in agg.values():
