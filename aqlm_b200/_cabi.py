@@ -92,6 +92,10 @@ def lib():
                 L.aqlm_b200_matmat_dequant_transposed.argtypes = [wp, vp, vp, i64, vp, ctypes.c_size_t, vp]
                 L.aqlm_b200_matmat_dequant_transposed_workspace_bytes.argtypes = [wp, i64]
                 L.aqlm_b200_matmat_dequant_transposed_workspace_bytes.restype = ctypes.c_size_t
+                L.aqlm_b200_matmat_dequant_grouped.argtypes = [wp, ctypes.POINTER(i64), ctypes.c_int, vp, vp, i64, u32, vp,
+                                                              ctypes.c_size_t, vp]
+                L.aqlm_b200_matmat_dequant_transposed_grouped.argtypes = [wp, ctypes.POINTER(i64), ctypes.c_int, vp, vp, i64,
+                                                                         vp, ctypes.c_size_t, vp]
                 L.aqlm_b200_scale_bias.argtypes = [vp, vp, vp, vp, i64, i64, i32, vp]
                 L.aqlm_b200_matmat_host.argtypes = [wp, vp, vp, vp, vp, i64, vp]
                 L.aqlm_b200_comm_shared_bytes.argtypes = [ctypes.c_int, i64]

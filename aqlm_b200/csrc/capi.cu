@@ -486,9 +486,21 @@ constexpr CUtensorMapDataType kTmapType = DT<T>::is_bf16 ? CU_TENSOR_MAP_DATA_TY
 // One launch of either GEMM.  Forward: b = x [batch][in_features], y [batch][out_features] (fp32 sums with `partial`).
 // TRANSPOSED (backward w.r.t. the input): b = grad_output [batch][out_features], y = grad_input [batch][in_features].
 // The directions differ in the code-tile map and in which side of W is the contraction; the rest is shared.
+// Segments of the out rows (GemmParams::n_seg / seg_end): one for a plain linear, up to 4 for a grouped call.
+struct GemmSegments {
+  int n_seg = 1;
+  int seg_end[4] = {0, 0, 0, 0};
+};
+
+static GemmSegments single_segment(const aqlm_b200_weight_t* w) {
+  GemmSegments s;
+  for (int& e : s.seg_end) e = (int)w->out_features;
+  return s;
+}
+
 template <typename T, int K, int CB, bool TRANSPOSED>
 static int launch_gemm(const aqlm_b200_weight_t* w, const void* b, void* y, int64_t batch, bool partial, const GemmPlan& g,
-                       void* workspace, const DeviceInfo* di, cudaStream_t st) {
+                       const GemmSegments& segs, void* workspace, const DeviceInfo* di, cudaStream_t st) {
   using Dir = std::conditional_t<TRANSPOSED, GemmTransposed<K, CB>, GemmForward<K, CB>>;
   const int64_t k_size = TRANSPOSED ? w->out_features : w->in_features;
   const size_t row_bytes = (size_t)(w->in_features / 8) * K * CB;
@@ -518,10 +530,17 @@ static int launch_gemm(const aqlm_b200_weight_t* w, const void* b, void* y, int6
   p.stages = g.stages;
   p.tile_m = g.tile_m;
   p.gather_mode = tun().gemm_gather_mode >= 0 ? tun().gemm_gather_mode : (w->nbits_per_codebook > 8 ? 1 : 0);
+  p.n_seg = segs.n_seg;
+  for (int i = 0; i < 4; ++i) p.seg_end[i] = segs.seg_end[i];
   return with_n_tile(g.n_tile, [&](auto N) {
+    const dim3 grid(g.m_tiles, g.ksplit, g.n_tiles);
+    const size_t smem = gemm_smem_layout(g.stages, N, Dir::kCtileBytes).total;
+    if (segs.n_seg > 1) {
+      constexpr auto kernel = TRANSPOSED ? gemm_dequant_t_grouped_kernel<T, K, CB, N> : gemm_dequant_grouped_kernel<T, K, CB, N>;
+      return launch<kernel>(di, grid, kGemmThreads, smem, st, 0, tb, tc, p);
+    }
     constexpr auto kernel = TRANSPOSED ? gemm_dequant_t_kernel<T, K, CB, N> : gemm_dequant_kernel<T, K, CB, N>;
-    return launch<kernel>(di, dim3(g.m_tiles, g.ksplit, g.n_tiles), kGemmThreads,
-                          gemm_smem_layout(g.stages, N, Dir::kCtileBytes).total, st, 0, tb, tc, p);
+    return launch<kernel>(di, grid, kGemmThreads, smem, st, 0, tb, tc, p);
   });
 }
 
@@ -541,6 +560,70 @@ static aqlm_b200_weight_t make_weight(const void* codes, const void* codebooks, 
   w.out_group_size = 1;
   w.dtype = dtype;
   return w;
+}
+
+// ---- grouped wgmma GEMM (forward and transposed): host side -----------------------------------------------------
+// Everything a grouped GEMM call checks without a device, in this order: arguments and segment table (ERR_SHAPE), then
+// the layouts the wgmma kernels take (ERR_UNSUPPORTED).  There is no GEMV form of a grouped call above 8 rows, so a
+// layout the kernels do not take is an error the caller handles (by running the members one by one).
+static int grouped_gemm_checks(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, const void* b,
+                               const void* y, int64_t batch, bool partial, bool transposed, GemmSegments* segs) {
+  int rc = validate(w, !partial);
+  if (rc) return rc;
+  if (batch < 0) return fail(AQLM_B200_ERR_SHAPE, "negative batch");
+  if (!b || !y) return fail(AQLM_B200_ERR_SHAPE, "input/output pointer is NULL");
+  if (!seg_rows || n_seg < 1 || n_seg > 4) return fail(AQLM_B200_ERR_SHAPE, "grouped GEMM takes 1..4 segments, got %d", n_seg);
+  int64_t acc = 0;
+  for (int i = 0; i < n_seg; ++i) {
+    if (seg_rows[i] <= 0) return fail(AQLM_B200_ERR_SHAPE, "segment %d has %lld rows", i, (long long)seg_rows[i]);
+    acc += seg_rows[i];
+    if (acc > w->out_features) break;
+    segs->seg_end[i] = (int)acc;
+  }
+  if (acc != w->out_features)
+    return fail(AQLM_B200_ERR_SHAPE, "segment rows do not add up to out_features (%lld)", (long long)w->out_features);
+  for (int i = n_seg; i < 4; ++i) segs->seg_end[i] = (int)acc;
+  segs->n_seg = n_seg;
+  const int K = w->num_codebooks, nbits = w->nbits_per_codebook, cb = nbits <= 8 ? 1 : 2;
+  if (w->in_group_size != 8 || (nbits != 8 && nbits != 16) || !(K == 1 || K == 2 || K == 4 || K == 8))
+    return fail(AQLM_B200_ERR_UNSUPPORTED,
+                "grouped GEMM covers in_group_size 8, 8/16-bit codes and 1/2/4/8 codebooks; got %dx%d, in_group_size %d",
+                K, nbits, w->in_group_size);
+  if (!transposed && w->in_features % kGemmBlockK != 0)
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped GEMM needs in_features %% 64 == 0, got %lld", (long long)w->in_features);
+  if (transposed && w->out_features % 8 != 0)
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped transposed GEMM needs out_features %% 8 == 0, got %lld",
+                (long long)w->out_features);
+  if (((size_t)(w->in_features / 8) * K * cb) % 16 != 0 || (reinterpret_cast<uintptr_t>(w->codes) & 15) != 0)
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped GEMM needs 16-byte aligned code rows");
+  if ((reinterpret_cast<uintptr_t>(b) & 15) != 0)
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped GEMM needs a 16-byte aligned %s", transposed ? "grad_output" : "input");
+  return AQLM_B200_OK;
+}
+
+// One launch of the forward (y [batch][out], fp32 sums with `partial`) or the transposed (y = grad_input [batch][in])
+// GEMM over the row-concatenated weight, with the plan of the concatenated descriptor.
+template <bool TRANSPOSED>
+static int grouped_gemm(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, const void* b, void* y,
+                        int64_t batch, bool partial, void* workspace, size_t workspace_bytes, void* stream) {
+  GemmSegments segs;
+  int rc = grouped_gemm_checks(w, seg_rows, n_seg, b, y, batch, partial, TRANSPOSED, &segs);
+  if (rc || batch == 0) return rc;
+  const DeviceInfo* di;
+  if ((rc = current_device(&di))) return rc;
+  const auto plan = [&](bool split) {
+    return TRANSPOSED ? gemm_t_plan(*w, batch, *di, tun(), split) : gemm_plan(*w, batch, *di, tun(), split);
+  };
+  GemmPlan g = plan(workspace != nullptr);
+  if (g.ok && g.ksplit > 1 && workspace_bytes < g.counters_bytes + g.partials_bytes) g = plan(false);
+  if (!g.ok) return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped GEMM: no wgmma plan for this descriptor and batch");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return with_dtype(w->dtype, [&](auto tag) {
+    return with_gemm_scheme(w, [&](auto K, auto CB) {
+      return launch_gemm<typename decltype(tag)::type, K, CB, TRANSPOSED>(w, b, y, batch, partial, g, segs, workspace, di,
+                                                                          st);
+    });
+  });
 }
 
 }  // namespace aqlm_b200
@@ -693,7 +776,8 @@ int aqlm_b200_matmat_dequant_ex(const aqlm_b200_weight_t* w, const void* input, 
   }
   return with_dtype(w->dtype, [&](auto tag) {
     return with_gemm_scheme(w, [&](auto K, auto CB) {
-      return launch_gemm<typename decltype(tag)::type, K, CB, false>(w, input, output, batch, partial, g, workspace, di, st);
+      return launch_gemm<typename decltype(tag)::type, K, CB, false>(w, input, output, batch, partial, g, single_segment(w),
+                                                             workspace, di, st);
     });
   });
 }
@@ -750,9 +834,23 @@ int aqlm_b200_matmat_dequant_transposed(const aqlm_b200_weight_t* w, const void*
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   return with_dtype(w->dtype, [&](auto tag) {
     return with_gemm_scheme(w, [&](auto K, auto CB) {
-      return launch_gemm<typename decltype(tag)::type, K, CB, true>(w, grad_output, grad_input, batch, false, g, workspace, di, st);
+      return launch_gemm<typename decltype(tag)::type, K, CB, true>(w, grad_output, grad_input, batch, false, g, single_segment(w),
+                                                            workspace, di, st);
     });
   });
+}
+
+int aqlm_b200_matmat_dequant_grouped(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, const void* input,
+                                     void* output, int64_t batch, uint32_t flags, void* workspace, size_t workspace_bytes,
+                                     void* stream) {
+  return grouped_gemm<false>(w, seg_rows, n_seg, input, output, batch, (flags & AQLM_B200_FLAG_PARTIAL_F32) != 0,
+                             workspace, workspace_bytes, stream);
+}
+
+int aqlm_b200_matmat_dequant_transposed_grouped(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg,
+                                                const void* grad_output, void* grad_input, int64_t batch, void* workspace,
+                                                size_t workspace_bytes, void* stream) {
+  return grouped_gemm<true>(w, seg_rows, n_seg, grad_output, grad_input, batch, false, workspace, workspace_bytes, stream);
 }
 
 int aqlm_b200_scale_bias(const float* partial, const void* scales, const void* bias, void* output, int64_t batch,

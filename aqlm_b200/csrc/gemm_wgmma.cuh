@@ -20,6 +20,9 @@
 // This file holds the pipeline itself (gemm_pipeline: shared-memory layout, barrier protocol, the three warp roles,
 // epilogue, split-K fix-up), written once for this kernel and for the transposed one of gemm_wgmma_t.cuh, and the
 // forward direction: GemmForward and gemm_dequant_kernel.  What a direction is, is listed at GemmForward.
+//
+// Grouped calls (q/k/v, gate/up: linears that read the same input): the weights are concatenated along the out rows
+// and GemmParams::n_seg / seg_end name the segments, each with its own stacked codebooks; one launch covers the group.
 #pragma once
 
 #include <type_traits>
@@ -59,7 +62,21 @@ struct GemmParams {
   int gather_mode;      // 0: ld.global.nc (L1 allocate), 1: ld.global.cg
   int partial_f32;      // forward only.  1: y is fp32 and gets the UNSCALED sums (no scale, no bias)
   int k_size;           // transposed only (scales of rows past it count as 0)
+  // grouped call (several linears sharing the input, out rows concatenated), as GemvParams: segment i covers out rows
+  // [seg_end[i-1], seg_end[i]) and its codebooks start at codebooks + i * (K << nbits) * 8 elements.  n_seg == 1: a
+  // plain linear.  scales / bias are concatenated like the rows, so the epilogue needs nothing per segment.
+  int n_seg;
+  int seg_end[4];
 };
+
+// Where the codebooks of the segment that owns out row `row` start, in 16-byte vectors from p.codebooks (rows past the
+// last segment end take the last segment's; seg_end[i] for i >= n_seg - 1 is the row count).  Branch-free on purpose:
+// the loop form `i < n_seg - 1 && row >= seg_end[i]` made ptxas keep GemmParams in local memory and spill.
+template <int K>
+__device__ __forceinline__ uint32_t gemm_segment_cb_offset(const GemmParams& p, int row) {
+  const uint32_t seg = (uint32_t)(row >= p.seg_end[0]) + (uint32_t)(row >= p.seg_end[1]) + (uint32_t)(row >= p.seg_end[2]);
+  return (min(seg, (uint32_t)p.n_seg - 1u) * K) << p.nbits;
+}
 
 // shared-memory carve-up (all offsets from a 1024-byte aligned base); ctile_bytes: one code-tile stage, a multiple of 16
 struct GemmSmem {
@@ -130,7 +147,8 @@ __device__ __forceinline__ void gemm_splitk_fixup(uint32_t* flag, unsigned int* 
 
 // The forward direction.  A direction is a compile-time description of everything the two GEMMs differ in: the A
 // operand's layout (descriptor on the consumer side, chunk addresses on the producer side), the code tile (TMA box,
-// where a producer thread finds its codes), the producer's thread mapping, and where the row scale is applied.
+// where a producer thread finds its codes), the producer's thread mapping (and the out row, hence the segment of a
+// grouped call, whose codes it dequantizes), and where the row scale is applied.
 // K = codebooks per group, CODE_BYTES = 1|2; in_group_size == 8.
 template <int K_, int CODE_BYTES_>
 struct GemmForward {
@@ -161,6 +179,10 @@ struct GemmForward {
   // producer thread pt -> (row pt / 2 of the tile, half pt % 2 of the 8 groups of a k-block)
   // rows past the (ragged) tile height: no gathers, nothing to write
   static __device__ __forceinline__ bool active(int pt, int tile_m) { return (pt >> 1) < tile_m; }
+  // the out row whose codes the thread dequantizes: the same tile row for every k-block, so a grouped call resolves
+  // its segment's codebooks once, before the k loop (a ragged tile may straddle a segment end: per row, not per tile)
+  static constexpr bool kRowPerKblock = false;
+  static __device__ __forceinline__ int out_row(int pt, int m0, int) { return m0 + (pt >> 1); }
   // byte 16 q of the thread's CB4 code bytes for k-block st_in of the staged tile: logical offset inside the 128-byte
   // code row -> physical (SWIZZLE_128B: 16-byte chunk ^= row & 7)
   static __device__ __forceinline__ int code_offset(int pt, int st_in, int q) {
@@ -175,8 +197,9 @@ struct GemmForward {
 };
 
 // The pipeline of both GEMM kernels; Dir is GemmForward or GemmTransposed, N the MMA width (columns of the batch tile).
-// tmap_b loads the K-major B operand (activations / grad_output), tmap_codes the code tiles.
-template <typename T, int N, typename Dir>
+// tmap_b loads the K-major B operand (activations / grad_output), tmap_codes the code tiles.  GROUPED: the kernel of
+// grouped calls (GemmParams::n_seg / seg_end); plain linears run kernels without any segment arithmetic.
+template <typename T, int N, typename Dir, bool GROUPED = false>
 __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const CUtensorMap& tmap_codes, const GemmParams& p) {
   constexpr int K = Dir::K, CODE_BYTES = Dir::CODE_BYTES, CB4 = Dir::CB4;
   constexpr int KB_PER_CTILE = Dir::kKbPerCtile;  // k-blocks covered by one code tile
@@ -333,6 +356,9 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
     const int pt = threadIdx.x - kGemmProducer0;
     const bool active = Dir::active(pt, TM);
     const uint4* gcb = reinterpret_cast<const uint4*>(p.codebooks);
+    // codebooks of the segment that owns the thread's out row (grouped calls only)
+    uint32_t cb_row = 0;
+    if constexpr (GROUPED && !Dir::kRowPerKblock) cb_row = gemm_segment_cb_offset<K>(p, Dir::out_row(pt, m0, 0));
     constexpr int CW = (CB4 + 3) / 4;        // 32-bit words holding the thread's CB4 code bytes
     constexpr bool INREG = K <= 2;           // hold the raw gathered vectors in registers until the write
     constexpr int KR = INREG ? K : 1;
@@ -348,6 +374,13 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
       const int ct = kb / KB_PER_CTILE, st_in = kb % KB_PER_CTILE;
       const int cs = (ct - ct0) % kCodeTileStages, cit = (ct - ct0) / kCodeTileStages;
       if constexpr (Dir::kScaleInProducer) sc = Dir::template row_scale<T>(p, pt, kb);
+      uint32_t cbo = cb_row;
+      if constexpr (GROUPED && Dir::kRowPerKblock) cbo = gemm_segment_cb_offset<K>(p, Dir::out_row(pt, m0, kb));
+      // codebook k's vector `code` (a plain linear: the first and only codebook set)
+      auto cb_vec = [&](int k, uint32_t code) -> const uint4* {
+        if constexpr (GROUPED) return gcb + (cbo + ((uint32_t)k << p.nbits) + code);
+        else return gcb + (((size_t)k << p.nbits) + code);
+      };
       mbar_wait(cfull_bar(cs), cit & 1);
       uint32_t cw[CW];
       const uint8_t* ctile = gbase + L.codes + cs * Dir::kCtileBytes;
@@ -374,15 +407,15 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
         if constexpr (INREG) {
 #pragma unroll
           for (int k = 0; k < K; ++k)
-            wv[e][k] = active ? gather(gcb + (((size_t)k << p.nbits) + code_at(e * K + k))) : make_uint4(0u, 0u, 0u, 0u);
+            wv[e][k] = active ? gather(cb_vec(k, code_at(e * K + k))) : make_uint4(0u, 0u, 0u, 0u);
         } else {
           float f[8];
 #pragma unroll
           for (int q = 0; q < 8; ++q) f[q] = 0.f;
           if (active) {
-            unpack8<T>(gather(gcb + code_at(e * K)), f);
+            unpack8<T>(gather(cb_vec(0, code_at(e * K))), f);
 #pragma unroll
-            for (int k = 1; k < K; ++k) accum8<T>(gather(gcb + (((size_t)k << p.nbits) + code_at(e * K + k))), f);
+            for (int k = 1; k < K; ++k) accum8<T>(gather(cb_vec(k, code_at(e * K + k))), f);
           }
           wv[e][0].x = DT<T>::pack2(f[0], f[1]); wv[e][0].y = DT<T>::pack2(f[2], f[3]);
           wv[e][0].z = DT<T>::pack2(f[4], f[5]); wv[e][0].w = DT<T>::pack2(f[6], f[7]);
@@ -475,6 +508,14 @@ template <typename T, int K, int CODE_BYTES, int N>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_dequant_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_codes, const GemmParams p) {
   gemm_pipeline<T, N, GemmForward<K, CODE_BYTES>>(tmap_x, tmap_codes, p);
+}
+
+// The same over the row-concatenated weights of a grouped call (q/k/v, gate/up: one launch for the group).
+template <typename T, int K, int CODE_BYTES, int N>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_dequant_grouped_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_codes,
+                            const GemmParams p) {
+  gemm_pipeline<T, N, GemmForward<K, CODE_BYTES>, true>(tmap_x, tmap_codes, p);
 }
 
 }  // namespace aqlm_b200

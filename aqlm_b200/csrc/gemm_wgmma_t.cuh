@@ -52,9 +52,12 @@ struct GemmTransposed {
 
   // producer thread pt -> (out row kk = pt / 4 of the k-block, groups 4 gq .. 4 gq + 3 of the tile's 16, gq = pt % 4)
   static __device__ __forceinline__ bool active(int, int) { return true; }
+  // the out row of the thread changes with every k-block: a grouped call resolves its segment's codebooks per k-block
+  static constexpr bool kRowPerKblock = true;
+  static __device__ __forceinline__ int out_row(int pt, int, int kb) { return kb * kGemmBlockK + (pt >> 2); }
   template <typename T>
   static __device__ __forceinline__ float row_scale(const GemmParams& p, int pt, int kb) {
-    const int o = kb * kGemmBlockK + (pt >> 2);
+    const int o = out_row(pt, 0, kb);
     return o < p.k_size ? DT<T>::to_float(reinterpret_cast<const T*>(p.scales)[o]) : 0.f;  // rows past the end contribute nothing
   }
   static __device__ __forceinline__ int code_offset(int pt, int st_in, int q) {
@@ -72,6 +75,14 @@ template <typename T, int K, int CODE_BYTES, int N>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_dequant_t_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_constant__ CUtensorMap tmap_codes, const GemmParams p) {
   gemm_pipeline<T, N, GemmTransposed<K, CODE_BYTES>>(tmap_g, tmap_codes, p);
+}
+
+// The backward of a grouped call: grad_output holds the members' output gradients side by side.
+template <typename T, int K, int CODE_BYTES, int N>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_dequant_t_grouped_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_constant__ CUtensorMap tmap_codes,
+                              const GemmParams p) {
+  gemm_pipeline<T, N, GemmTransposed<K, CODE_BYTES>, true>(tmap_g, tmap_codes, p);
 }
 
 }  // namespace aqlm_b200

@@ -8,8 +8,9 @@ grouped launches wired into a loaded model.
   `AutoModelForCausalLM.from_pretrained(dir)` then builds `aqlm.QuantizedLinear` modules through Hugging Face's own AQLM
   integration (`transformers/integrations/aqlm.py`) -- with `aqlm_b200.install_as_aqlm()` those are OUR modules.
 * `fuse_shared_input_linears` finds, in a loaded model, the quantized linears that read the same activation (attention
-  q/k/v, MLP gate/up) and makes each set run as ONE grouped launch (`QuantizedLinearGroup`), without changing module
-  names, the state dict, or the model's forward code: the members' `forward` is routed through a small per-group cache.
+  q/k/v, MLP gate/up) and makes each set run as ONE grouped launch (`QuantizedLinearGroup`: the grouped GEMV at decode,
+  the grouped GEMM at prefill and in training), without changing module names, the state dict, or the model's forward
+  code: the members' `forward` is routed through a small per-group cache.
 """
 from __future__ import annotations
 
@@ -21,7 +22,7 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 import torch
 from torch import nn
 
-from .grouped import QuantizedLinearGroup
+from .grouped import QuantizedLinearGroup, _rows, gemm_scheme
 from .inference import QuantizedLinear
 from .utils import pack_int_data
 
@@ -39,15 +40,19 @@ class _SharedInputGroup:
         self._version = -1
         self._outs: Optional[Tuple[torch.Tensor, ...]] = None
         self._left = 0
+        self._in_group = False
 
     def member_forward(self, index: int, member: QuantizedLinear, x: torch.Tensor) -> torch.Tensor:
-        rows = 1
-        for d in x.shape[:-1]:
-            rows *= d
-        if not self.group.fused or rows > 8 or rows < 1 or (torch.is_grad_enabled() and x.requires_grad):
-            return QuantizedLinear.forward(member, x)  # large batch / training: the member's own op
+        rows = _rows(x)
+        # the group's own fallback to its members (a layout no grouped kernel takes) lands here: the member's own op
+        if self._in_group or not self.group.fused or rows < 1:
+            return QuantizedLinear.forward(member, x)
         if self._x is not x or self._version != x._version:  # a new activation (or the same tensor modified in place)
-            self._outs = self.group(x)
+            self._in_group = True
+            try:
+                self._outs = self.group(x)  # decode, prefill and training: one grouped launch where a kernel takes it
+            finally:
+                self._in_group = False
             self._x, self._version, self._left = x, x._version, len(self._outs)
         y = self._outs[index]
         self._left -= 1
@@ -69,7 +74,7 @@ def fuse_shared_input_linears(model: nn.Module, sets: Iterable[Sequence[str]] = 
             if any(getattr(m, "_aqlm_b200_group", None) is not None for m in members):
                 continue
             m0 = members[0]
-            if not m0.codes.is_cuda or (m0.num_codebooks, m0.nbits_per_codebook, m0.in_group_size) != (1, 16, 8):
+            if not m0.codes.is_cuda or not gemm_scheme(m0):
                 continue
             if any(m.in_features != m0.in_features or (m.bias is None) != (m0.bias is None) for m in members):
                 continue

@@ -213,6 +213,76 @@ def matmat_grouped(input, codes, codebooks_stacked, scales, bias, seg_rows, part
     return out.reshape(input.shape[:-1] + (w.out_features,))
 
 
+def _grouped_weight(codes, codebooks_stacked, scales, bias, seg_rows):
+    n_seg = codebooks_stacked.shape[0]
+    if n_seg != len(seg_rows) or not codebooks_stacked.is_contiguous():
+        raise ValueError("codebooks_stacked must be a contiguous [n_seg, ...] stack matching seg_rows")
+    w = make_weight(codes, codebooks_stacked[0], scales.reshape(-1) if scales is not None else None, bias)
+    return w, (ctypes.c_int64 * n_seg)(*[int(r) for r in seg_rows]), n_seg
+
+
+def matmat_dequant_grouped(input, codes, codebooks_stacked, scales, bias, seg_rows,
+                           partial: bool = False) -> Optional[torch.Tensor]:
+    """ONE wgmma GEMM launch for several linears sharing `input`, any batch and any scheme the GEMM covers: `codes`
+    [sum(seg_rows), in/8, K] (row-concatenated), `codebooks_stacked` [n_seg, K, 2^nbits, 1, 8], `scales`/`bias`
+    concatenated.  Returns [..., sum(seg_rows)] in the input dtype, or UNSCALED fp32 sums when `partial`.  Returns None
+    when the library does not take the layout (ERR_UNSUPPORTED): the caller then runs the members."""
+    device = _require_cuda(input, codes, codebooks_stacked, scales, bias)
+    _dtype_code(input)
+    if input.dtype != codebooks_stacked.dtype:
+        raise ValueError(f"input dtype {input.dtype} != codebooks dtype {codebooks_stacked.dtype}")
+    w, seg, n_seg = _grouped_weight(codes, codebooks_stacked, None if partial else scales, None if partial else bias,
+                                    seg_rows)
+    if input.shape[-1] != w.in_features:
+        raise ValueError(f"input has {input.shape[-1]} features, weight expects {w.in_features}")
+    flat = input.reshape(-1, input.shape[-1])
+    if not flat.is_contiguous():
+        flat = flat.contiguous()
+    batch = flat.shape[0]
+    out = torch.empty((batch, w.out_features), dtype=torch.float32 if partial else input.dtype, device=device)
+    with _on_device(device):
+        L = _cabi.lib()
+        need = L.aqlm_b200_matmat_dequant_workspace_bytes(ctypes.byref(w), batch) if batch > 0 else 0
+        ws = _workspace(device, need) if need else None
+        rc = L.aqlm_b200_matmat_dequant_grouped(ctypes.byref(w), seg, n_seg, flat.data_ptr(), out.data_ptr(), batch,
+                                                _cabi.FLAG_PARTIAL_F32 if partial else 0,
+                                                ws.data_ptr() if ws is not None else None,
+                                                ws.numel() if ws is not None else 0, _stream_ptr(device))
+    if rc == _cabi.ERR_UNSUPPORTED:
+        return None
+    _cabi.check(rc)
+    return out.reshape(input.shape[:-1] + (w.out_features,))
+
+
+def matmat_dequant_transposed_grouped(grad_out, codes, codebooks_stacked, scales, seg_rows) -> Optional[torch.Tensor]:
+    """Backward w.r.t. the input of a group in ONE transposed wgmma GEMM: grad_in = (grad_out * scales) @ W over the
+    row-concatenated weight, `grad_out` [..., sum(seg_rows)] (the group's concatenated output gradient).  Returns None
+    when the library does not take the layout (ERR_UNSUPPORTED)."""
+    device = _require_cuda(grad_out, codes, codebooks_stacked, scales)
+    _dtype_code(grad_out)
+    if grad_out.dtype != codebooks_stacked.dtype:
+        raise ValueError(f"grad_output dtype {grad_out.dtype} != codebooks dtype {codebooks_stacked.dtype}")
+    w, seg, n_seg = _grouped_weight(codes, codebooks_stacked, scales, None, seg_rows)
+    if grad_out.shape[-1] != w.out_features:
+        raise ValueError(f"grad_output has {grad_out.shape[-1]} features, weight has {w.out_features} output rows")
+    flat = grad_out.reshape(-1, grad_out.shape[-1])
+    if not flat.is_contiguous():
+        flat = flat.contiguous()
+    batch = flat.shape[0]
+    out = torch.empty((batch, w.in_features), dtype=grad_out.dtype, device=device)
+    with _on_device(device):
+        L = _cabi.lib()
+        need = L.aqlm_b200_matmat_dequant_transposed_workspace_bytes(ctypes.byref(w), batch) if batch > 0 else 0
+        ws = _workspace(device, need) if need else None
+        rc = L.aqlm_b200_matmat_dequant_transposed_grouped(ctypes.byref(w), seg, n_seg, flat.data_ptr(), out.data_ptr(),
+                                                           batch, ws.data_ptr() if ws is not None else None,
+                                                           ws.numel() if ws is not None else 0, _stream_ptr(device))
+    if rc == _cabi.ERR_UNSUPPORTED:
+        return None
+    _cabi.check(rc)
+    return out.reshape(grad_out.shape[:-1] + (w.in_features,))
+
+
 def matmat_partial(input, codes, codebooks) -> torch.Tensor:
     """UNSCALED fp32 partial products [batch, out] of an in_features shard (to be all-reduced).  Above GEMV_MAX_ROWS
     rows (prefill) this is the wgmma GEMM, as in QuantizedLinear; below, the GEMV / LUT kernels."""

@@ -127,6 +127,26 @@ size_t aqlm_b200_matmat_dequant_transposed_workspace_bytes(const aqlm_b200_weigh
 int aqlm_b200_matmat_dequant_transposed(const aqlm_b200_weight_t* w, const void* grad_output, void* grad_input,
                                         int64_t batch, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Grouped form of the two tensor-core GEMMs above, for linears that share their input (q/k/v, gate/up) at any batch:
+ * ONE launch over the row-concatenated weight.  `w`, `seg_rows` and `n_seg` describe the group as for
+ * aqlm_b200_matmat_grouped: codes [sum(seg_rows), in/in_group, K], scales/bias [sum(seg_rows)], and w->codebooks
+ * points to n_seg codebook sets stacked back to back (K * 2^nbits * 8 elements each).  The plan is the one of the
+ * concatenated descriptor, so aqlm_b200_matmat_dequant[_transposed]_workspace_bytes(w, batch) gives the workspace.
+ *   forward:     output [batch, sum(seg_rows)]; flags as for aqlm_b200_matmat_dequant_ex (AQLM_B200_FLAG_PARTIAL_F32:
+ *                fp32 unscaled sums, scales/bias may be NULL).
+ *   transposed:  grad_input [batch, in] = (grad_output [batch, sum(seg_rows)] * scales) @ W_concatenated.
+ * Any scheme the tensor-core kernels cover: in_group_size 8, 8/16-bit codes, 1/2/4/8 codebooks, 16-byte aligned code
+ * rows and input, and in_features % 64 == 0 (forward) or out_features % 8 == 0 (transposed).  Anything else returns
+ * AQLM_B200_ERR_UNSUPPORTED: unlike aqlm_b200_matmat_dequant_ex there is no GEMV form to fall back to, so the caller
+ * runs the members one by one.  n_seg outside 1..4, an empty segment, or rows that do not add up to out_features:
+ * AQLM_B200_ERR_SHAPE.  Both checks come before any device query. */
+int aqlm_b200_matmat_dequant_grouped(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, const void* input,
+                                     void* output, int64_t batch, uint32_t flags, void* workspace, size_t workspace_bytes,
+                                     void* stream);
+int aqlm_b200_matmat_dequant_transposed_grouped(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg,
+                                                const void* grad_output, void* grad_input, int64_t batch, void* workspace,
+                                                size_t workspace_bytes, void* stream);
+
 /* Epilogue of the sharded path: output[b,o] = (T)(partial[b,o] * scales[o] + bias[o]) after the
  * all-reduce of the fp32 partials (new work; the reference has no multi-GPU hot path, SURVEY §8e). */
 int aqlm_b200_scale_bias(const float* partial, const void* scales, const void* bias, void* output, int64_t batch,
