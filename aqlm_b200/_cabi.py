@@ -96,6 +96,13 @@ def lib():
                                                               ctypes.c_size_t, vp]
                 L.aqlm_b200_matmat_dequant_transposed_grouped.argtypes = [wp, ctypes.POINTER(i64), ctypes.c_int, vp, vp, i64,
                                                                          vp, ctypes.c_size_t, vp]
+                L.aqlm_b200_matmat_dequant_routed_workspace_bytes.argtypes = [wp, ctypes.c_int, i64, ctypes.c_int]
+                L.aqlm_b200_matmat_dequant_routed_workspace_bytes.restype = ctypes.c_size_t
+                L.aqlm_b200_matmat_dequant_routed.argtypes = [wp, ctypes.POINTER(i64), ctypes.c_int, ctypes.c_int, vp, vp,
+                                                             vp, i64, vp, ctypes.c_size_t, vp]
+                L.aqlm_b200_matmat_dequant_transposed_routed.argtypes = [wp, ctypes.POINTER(i64), ctypes.c_int,
+                                                                        ctypes.c_int, vp, vp, vp, i64, vp,
+                                                                        ctypes.c_size_t, vp]
                 L.aqlm_b200_scale_bias.argtypes = [vp, vp, vp, vp, i64, i64, i32, vp]
                 L.aqlm_b200_matmat_host.argtypes = [wp, vp, vp, vp, vp, i64, vp]
                 L.aqlm_b200_comm_shared_bytes.argtypes = [ctypes.c_int, i64]

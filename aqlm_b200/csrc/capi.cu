@@ -498,9 +498,11 @@ static GemmSegments single_segment(const aqlm_b200_weight_t* w) {
   return s;
 }
 
+// A routed call (expert_off != NULL) covers n_experts stacked experts of w's shape: the code map spans all of them.
 template <typename T, int K, int CB, bool TRANSPOSED>
 static int launch_gemm(const aqlm_b200_weight_t* w, const void* b, void* y, int64_t batch, bool partial, const GemmPlan& g,
-                       const GemmSegments& segs, void* workspace, const DeviceInfo* di, cudaStream_t st) {
+                       const GemmSegments& segs, void* workspace, const DeviceInfo* di, cudaStream_t st,
+                       const int32_t* expert_off = nullptr, int n_experts = 1) {
   using Dir = std::conditional_t<TRANSPOSED, GemmTransposed<K, CB>, GemmForward<K, CB>>;
   const int64_t k_size = TRANSPOSED ? w->out_features : w->in_features;
   const size_t row_bytes = (size_t)(w->in_features / 8) * K * CB;
@@ -508,9 +510,10 @@ static int launch_gemm(const aqlm_b200_weight_t* w, const void* b, void* y, int6
   if (int rc = encode_tmap(&tb, TRANSPOSED ? "grad_output" : "x", kTmapType<T>, b, k_size, batch, k_size * 2, kGemmBlockK,
                            g.n_tile, CU_TENSOR_MAP_SWIZZLE_128B))
     return rc;
+  const uint64_t code_rows = (uint64_t)w->out_features * (uint64_t)n_experts;
   if (int rc = TRANSPOSED ? encode_tmap(&tc, "codes, transposed", CU_TENSOR_MAP_DATA_TYPE_UINT8, w->codes, row_bytes,
-                                        w->out_features, row_bytes, 16 * K * CB, kGemmTCtileRows, CU_TENSOR_MAP_SWIZZLE_NONE)
-                          : encode_tmap(&tc, "codes", CU_TENSOR_MAP_DATA_TYPE_UINT8, w->codes, row_bytes, w->out_features,
+                                        code_rows, row_bytes, 16 * K * CB, kGemmTCtileRows, CU_TENSOR_MAP_SWIZZLE_NONE)
+                          : encode_tmap(&tc, "codes", CU_TENSOR_MAP_DATA_TYPE_UINT8, w->codes, row_bytes, code_rows,
                                         row_bytes, kCodeTileBytes, g.tile_m, CU_TENSOR_MAP_SWIZZLE_128B))
     return rc;
   GemmParams p;
@@ -532,9 +535,15 @@ static int launch_gemm(const aqlm_b200_weight_t* w, const void* b, void* y, int6
   p.gather_mode = tun().gemm_gather_mode >= 0 ? tun().gemm_gather_mode : (w->nbits_per_codebook > 8 ? 1 : 0);
   p.n_seg = segs.n_seg;
   for (int i = 0; i < 4; ++i) p.seg_end[i] = segs.seg_end[i];
+  p.expert_off = expert_off;
+  p.n_experts = n_experts;
   return with_n_tile(g.n_tile, [&](auto N) {
-    const dim3 grid(g.m_tiles, g.ksplit, g.n_tiles);
+    const dim3 grid(g.m_tiles, g.ksplit, g.n_tiles);  // routed: n_tiles is the slot count
     const size_t smem = gemm_smem_layout(g.stages, N, Dir::kCtileBytes).total;
+    if (expert_off) {
+      constexpr auto kernel = TRANSPOSED ? gemm_dequant_t_routed_kernel<T, K, CB, N> : gemm_dequant_routed_kernel<T, K, CB, N>;
+      return launch<kernel>(di, grid, kGemmThreads, smem, st, 0, tb, tc, p);
+    }
     if (segs.n_seg > 1) {
       constexpr auto kernel = TRANSPOSED ? gemm_dequant_t_grouped_kernel<T, K, CB, N> : gemm_dequant_grouped_kernel<T, K, CB, N>;
       return launch<kernel>(di, grid, kGemmThreads, smem, st, 0, tb, tc, p);
@@ -566,13 +575,10 @@ static aqlm_b200_weight_t make_weight(const void* codes, const void* codebooks, 
 // Everything a grouped GEMM call checks without a device, in this order: arguments and segment table (ERR_SHAPE), then
 // the layouts the wgmma kernels take (ERR_UNSUPPORTED).  There is no GEMV form of a grouped call above 8 rows, so a
 // layout the kernels do not take is an error the caller handles (by running the members one by one).
-static int grouped_gemm_checks(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, const void* b,
-                               const void* y, int64_t batch, bool partial, bool transposed, GemmSegments* segs) {
-  int rc = validate(w, !partial);
-  if (rc) return rc;
-  if (batch < 0) return fail(AQLM_B200_ERR_SHAPE, "negative batch");
-  if (!b || !y) return fail(AQLM_B200_ERR_SHAPE, "input/output pointer is NULL");
-  if (!seg_rows || n_seg < 1 || n_seg > 4) return fail(AQLM_B200_ERR_SHAPE, "grouped GEMM takes 1..4 segments, got %d", n_seg);
+// The segment table of a grouped or routed call (ERR_SHAPE).
+static int gemm_segment_table(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, const char* what,
+                              GemmSegments* segs) {
+  if (!seg_rows || n_seg < 1 || n_seg > 4) return fail(AQLM_B200_ERR_SHAPE, "%s GEMM takes 1..4 segments, got %d", what, n_seg);
   int64_t acc = 0;
   for (int i = 0; i < n_seg; ++i) {
     if (seg_rows[i] <= 0) return fail(AQLM_B200_ERR_SHAPE, "segment %d has %lld rows", i, (long long)seg_rows[i]);
@@ -584,21 +590,37 @@ static int grouped_gemm_checks(const aqlm_b200_weight_t* w, const int64_t* seg_r
     return fail(AQLM_B200_ERR_SHAPE, "segment rows do not add up to out_features (%lld)", (long long)w->out_features);
   for (int i = n_seg; i < 4; ++i) segs->seg_end[i] = (int)acc;
   segs->n_seg = n_seg;
+  return AQLM_B200_OK;
+}
+
+// The layouts the wgmma kernels of a grouped or routed call take (ERR_UNSUPPORTED otherwise).
+static int gemm_layout_checks(const aqlm_b200_weight_t* w, const void* b, bool transposed, const char* what) {
   const int K = w->num_codebooks, nbits = w->nbits_per_codebook, cb = nbits <= 8 ? 1 : 2;
   if (w->in_group_size != 8 || (nbits != 8 && nbits != 16) || !(K == 1 || K == 2 || K == 4 || K == 8))
     return fail(AQLM_B200_ERR_UNSUPPORTED,
-                "grouped GEMM covers in_group_size 8, 8/16-bit codes and 1/2/4/8 codebooks; got %dx%d, in_group_size %d",
-                K, nbits, w->in_group_size);
+                "%s GEMM covers in_group_size 8, 8/16-bit codes and 1/2/4/8 codebooks; got %dx%d, in_group_size %d",
+                what, K, nbits, w->in_group_size);
   if (!transposed && w->in_features % kGemmBlockK != 0)
-    return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped GEMM needs in_features %% 64 == 0, got %lld", (long long)w->in_features);
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s GEMM needs in_features %% 64 == 0, got %lld", what,
+                (long long)w->in_features);
   if (transposed && w->out_features % 8 != 0)
-    return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped transposed GEMM needs out_features %% 8 == 0, got %lld",
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s transposed GEMM needs out_features %% 8 == 0, got %lld", what,
                 (long long)w->out_features);
   if (((size_t)(w->in_features / 8) * K * cb) % 16 != 0 || (reinterpret_cast<uintptr_t>(w->codes) & 15) != 0)
-    return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped GEMM needs 16-byte aligned code rows");
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s GEMM needs 16-byte aligned code rows", what);
   if ((reinterpret_cast<uintptr_t>(b) & 15) != 0)
-    return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped GEMM needs a 16-byte aligned %s", transposed ? "grad_output" : "input");
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s GEMM needs a 16-byte aligned %s", what, transposed ? "grad_output" : "input");
   return AQLM_B200_OK;
+}
+
+static int grouped_gemm_checks(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, const void* b,
+                               const void* y, int64_t batch, bool partial, bool transposed, GemmSegments* segs) {
+  int rc = validate(w, !partial);
+  if (rc) return rc;
+  if (batch < 0) return fail(AQLM_B200_ERR_SHAPE, "negative batch");
+  if (!b || !y) return fail(AQLM_B200_ERR_SHAPE, "input/output pointer is NULL");
+  if ((rc = gemm_segment_table(w, seg_rows, n_seg, "grouped", segs))) return rc;
+  return gemm_layout_checks(w, b, transposed, "grouped");
 }
 
 // One launch of the forward (y [batch][out], fp32 sums with `partial`) or the transposed (y = grad_input [batch][in])
@@ -622,6 +644,52 @@ static int grouped_gemm(const aqlm_b200_weight_t* w, const int64_t* seg_rows, in
     return with_gemm_scheme(w, [&](auto K, auto CB) {
       return launch_gemm<typename decltype(tag)::type, K, CB, TRANSPOSED>(w, b, y, batch, partial, g, segs, workspace, di,
                                                                           st);
+    });
+  });
+}
+
+// ---- routed wgmma GEMM (mixture-of-experts, forward and transposed): host side -----------------------------------
+constexpr int kRoutedMaxExperts = 64;
+
+// Everything a routed call checks without a device, in this order: descriptor, segment table, expert count, pointers
+// (ERR_SHAPE); then the layouts the wgmma kernels take (ERR_UNSUPPORTED), exactly as for a grouped call.
+static int routed_gemm_checks(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, int n_experts,
+                              const int32_t* expert_off, const void* b, const void* y, int64_t rows, bool transposed,
+                              GemmSegments* segs) {
+  int rc = validate(w, true);
+  if (rc) return rc;
+  if (rows < 0) return fail(AQLM_B200_ERR_SHAPE, "negative row count");
+  if (rows > 0x7fffffffll) return fail(AQLM_B200_ERR_SHAPE, "routed GEMM takes at most 2^31 - 1 rows");
+  const int64_t one[1] = {w->out_features};
+  if ((rc = gemm_segment_table(w, (seg_rows || n_seg != 1) ? seg_rows : one, n_seg, "routed", segs))) return rc;
+  if (n_experts < 1 || n_experts > kRoutedMaxExperts)
+    return fail(AQLM_B200_ERR_SHAPE, "routed GEMM takes 1..%d experts, got %d", kRoutedMaxExperts, n_experts);
+  if (w->out_features * n_experts > 0x7fffffffll)  // the stacked out rows are a TMA coordinate
+    return fail(AQLM_B200_ERR_SHAPE, "routed GEMM: %d experts x %lld out rows exceed 2^31 - 1", n_experts,
+                (long long)w->out_features);
+  if (!expert_off) return fail(AQLM_B200_ERR_SHAPE, "expert offsets pointer is NULL");
+  if (!b || !y) return fail(AQLM_B200_ERR_SHAPE, "input/output pointer is NULL");
+  return gemm_layout_checks(w, b, transposed, "routed");
+}
+
+template <bool TRANSPOSED>
+static int routed_gemm(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, int n_experts,
+                       const int32_t* expert_off, const void* b, void* y, int64_t rows, void* workspace,
+                       size_t workspace_bytes, void* stream) {
+  GemmSegments segs;
+  int rc = routed_gemm_checks(w, seg_rows, n_seg, n_experts, expert_off, b, y, rows, TRANSPOSED, &segs);
+  if (rc || rows == 0) return rc;
+  const DeviceInfo* di;
+  if ((rc = current_device(&di))) return rc;
+  const auto plan = [&](bool split) { return gemm_routed_plan(*w, rows, n_experts, *di, tun(), split, TRANSPOSED); };
+  GemmPlan g = plan(workspace != nullptr);
+  if (g.ok && g.ksplit > 1 && workspace_bytes < g.counters_bytes + g.partials_bytes) g = plan(false);
+  if (!g.ok) return fail(AQLM_B200_ERR_UNSUPPORTED, "routed GEMM: no wgmma plan for this descriptor and row count");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return with_dtype(w->dtype, [&](auto tag) {
+    return with_gemm_scheme(w, [&](auto K, auto CB) {
+      return launch_gemm<typename decltype(tag)::type, K, CB, TRANSPOSED>(w, b, y, rows, false, g, segs, workspace, di,
+                                                                          st, expert_off, n_experts);
     });
   });
 }
@@ -851,6 +919,31 @@ int aqlm_b200_matmat_dequant_transposed_grouped(const aqlm_b200_weight_t* w, con
                                                 const void* grad_output, void* grad_input, int64_t batch, void* workspace,
                                                 size_t workspace_bytes, void* stream) {
   return grouped_gemm<true>(w, seg_rows, n_seg, grad_output, grad_input, batch, false, workspace, workspace_bytes, stream);
+}
+
+size_t aqlm_b200_matmat_dequant_routed_workspace_bytes(const aqlm_b200_weight_t* w, int n_experts, int64_t rows,
+                                                       int transposed) {
+  if (validate(w, false) != AQLM_B200_OK || rows <= 0 || n_experts < 1 || n_experts > kRoutedMaxExperts) return 0;
+  const DeviceInfo* di = device_info();
+  if (!di) return 0;
+  const GemmPlan g = gemm_routed_plan(*w, rows, n_experts, *di, tun(), true, transposed != 0);
+  if (!g.ok || g.ksplit <= 1) return 0;
+  return g.counters_bytes + g.partials_bytes;
+}
+
+int aqlm_b200_matmat_dequant_routed(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, int n_experts,
+                                    const int32_t* expert_offsets, const void* input, void* output, int64_t rows,
+                                    void* workspace, size_t workspace_bytes, void* stream) {
+  return routed_gemm<false>(w, seg_rows, n_seg, n_experts, expert_offsets, input, output, rows, workspace,
+                            workspace_bytes, stream);
+}
+
+int aqlm_b200_matmat_dequant_transposed_routed(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg,
+                                               int n_experts, const int32_t* expert_offsets, const void* grad_output,
+                                               void* grad_input, int64_t rows, void* workspace, size_t workspace_bytes,
+                                               void* stream) {
+  return routed_gemm<true>(w, seg_rows, n_seg, n_experts, expert_offsets, grad_output, grad_input, rows, workspace,
+                           workspace_bytes, stream);
 }
 
 int aqlm_b200_scale_bias(const float* partial, const void* scales, const void* bias, void* output, int64_t batch,

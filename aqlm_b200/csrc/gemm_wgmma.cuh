@@ -23,11 +23,19 @@
 //
 // Grouped calls (q/k/v, gate/up: linears that read the same input): the weights are concatenated along the out rows
 // and GemmParams::n_seg / seg_end name the segments, each with its own stacked codebooks; one launch covers the group.
+//
+// Routed calls (mixture-of-experts: E experts of one shape, each applied to its own run of the input rows, which are
+// sorted by expert): one launch covers every expert.  The grid's third index is a slot, not a batch tile; a CTA
+// resolves it to (expert, first row, end row) from the device-side expert offsets (routing.cuh) and offsets its code
+// tiles, codebooks, scales and bias by the expert.  PDL: the offsets are written by the previous kernel, so a routed
+// CTA waits for it (griddep_wait) before it knows its expert, and its weight-side prologue (code tiles, gathers) no
+// longer overlaps the previous kernel's tail as the plain and grouped kernels' does.
 #pragma once
 
 #include <type_traits>
 
 #include "gemm_wgmma_ptx.cuh"
+#include "routing.cuh"
 
 namespace aqlm_b200 {
 
@@ -67,6 +75,11 @@ struct GemmParams {
   // plain linear.  scales / bias are concatenated like the rows, so the epilogue needs nothing per segment.
   int n_seg;
   int seg_end[4];
+  // routed call: expert e covers input / output rows [expert_off[e], expert_off[e+1]) (clamped, see routing.cuh) and
+  // owns out rows [e * out, (e + 1) * out) of the stacked codes, scales and bias and codebook sets [e * n_seg, (e + 1) *
+  // n_seg).  batch is the total row count.  Unused by plain and grouped calls.
+  const int* expert_off;
+  int n_experts;
 };
 
 // Where the codebooks of the segment that owns out row `row` start, in 16-byte vectors from p.codebooks (rows past the
@@ -167,6 +180,8 @@ struct GemmForward {
   // Scale (and bias) are applied to the sums in the epilogue / the split-K fix-up; tiles may be ragged (tile_m < 128).
   static constexpr bool kScaleInProducer = false;
   static __device__ __forceinline__ int tile_m(const GemmParams& p) { return p.tile_m; }
+  // out rows of one expert of a routed call (the forward's output rows)
+  static __device__ __forceinline__ int out_rows(const GemmParams& p) { return p.m_size; }
 
   // code tile: tile_m rows x 128 bytes of codes, SWIZZLE_128B; covers kKbPerCtile k-blocks
   static constexpr int kCtileBytes = kGemmBlockM * kCodeTileBytes;
@@ -198,9 +213,11 @@ struct GemmForward {
 
 // The pipeline of both GEMM kernels; Dir is GemmForward or GemmTransposed, N the MMA width (columns of the batch tile).
 // tmap_b loads the K-major B operand (activations / grad_output), tmap_codes the code tiles.  GROUPED: the kernel of
-// grouped calls (GemmParams::n_seg / seg_end); plain linears run kernels without any segment arithmetic.
-template <typename T, int N, typename Dir, bool GROUPED = false>
+// grouped calls (GemmParams::n_seg / seg_end); plain linears run kernels without any segment arithmetic.  ROUTED (with
+// GROUPED): the kernel of routed calls (GemmParams::expert_off / n_experts); see the file comment.
+template <typename T, int N, typename Dir, bool GROUPED = false, bool ROUTED = false>
 __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const CUtensorMap& tmap_codes, const GemmParams& p) {
+  static_assert(!ROUTED || GROUPED, "a routed kernel resolves segments too");
   constexpr int K = Dir::K, CODE_BYTES = Dir::CODE_BYTES, CB4 = Dir::CB4;
   constexpr int KB_PER_CTILE = Dir::kKbPerCtile;  // k-blocks covered by one code tile
   static_assert(KB_PER_CTILE >= 1, "scheme too wide for the code tile");
@@ -213,11 +230,26 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_tile = blockIdx.x, split = blockIdx.y, n_blk = blockIdx.z;
-  const int m0 = m_tile * TM, n0 = n_blk * N;
+  const int m0 = m_tile * TM;
   // PDL: the next kernel of the stream may be dispatched as soon as SM resources free up (no launch gap).  Everything this
   // kernel does before griddep_wait() touches WEIGHTS only (code tiles, codebook gathers, scales); the B tiles are read
   // and y / the workspace written after it.
   griddep_launch_dependents();
+  // Columns of the tile: batch rows [n0, n0 + N), valid below n_end().  A routed CTA takes them, and its expert, from
+  // its slot; the expert's weights start e_rows out rows (and e_cb codebook vectors) into the stacks.  Plain and grouped
+  // kernels read p.batch where they always did (a local copy of it changed their register allocation).
+  RoutedSlot rs{0, 0, 0};
+  size_t e_rows = 0;
+  uint32_t e_cb = 0;
+  if constexpr (ROUTED) {
+    griddep_wait();  // the offsets are the previous kernel's output
+    rs = routed_slot(p.expert_off, p.n_experts, p.batch, N, n_blk);
+    if (rs.expert < 0) return;  // past the last tile: no barrier, no workspace touched
+    e_rows = (size_t)rs.expert * Dir::out_rows(p);
+    e_cb = ((uint32_t)rs.expert * (uint32_t)p.n_seg * K) << p.nbits;
+  }
+  const int n0 = ROUTED ? rs.row0 : n_blk * N;
+  auto n_end = [&]() { return ROUTED ? rs.row1 : p.batch; };
   // k-block range of this split (balanced, contiguous)
   const int kb0 = (int)(((long long)p.total_kblocks * split) / p.ksplit);
   const int kb1 = (int)(((long long)p.total_kblocks * (split + 1)) / p.ksplit);
@@ -290,8 +322,8 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
       float sc = 1.f, bi = 0.f;
       if constexpr (!Dir::kScaleInProducer) {
         if (row_ok && p.ksplit == 1 && !p.partial_f32) {
-          sc = DT<T>::to_float(reinterpret_cast<const T*>(p.scales)[row]);
-          if (p.bias) bi = DT<T>::to_float(reinterpret_cast<const T*>(p.bias)[row]);
+          sc = DT<T>::to_float((reinterpret_cast<const T*>(p.scales) + e_rows)[row]);
+          if (p.bias) bi = DT<T>::to_float((reinterpret_cast<const T*>(p.bias) + e_rows)[row]);
         }
       }
 #pragma unroll
@@ -301,7 +333,7 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
           const int col = 8 * i + 2 * (lane & 3) + c;
           const float v = acc[4 * i + 2 * j + c];
           if (p.ksplit == 1) {
-            if (row_ok && n0 + col < p.batch) {
+            if (row_ok && n0 + col < n_end()) {
               const size_t o = (size_t)(n0 + col) * p.m_size + row;
               if constexpr (Dir::kScaleInProducer) {
                 y[o] = DT<T>::from_float(v);
@@ -328,7 +360,7 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
         if (elect_one()) {
           const int2 at = Dir::ctile_coord(m_tile, TM, ct);
           mbar_expect_tx(cfull_bar(cs), Dir::ctile_tx_bytes(TM));
-          tma_load_2d(base + L.codes + cs * Dir::kCtileBytes, &tmap_codes, at.x, at.y, cfull_bar(cs));
+          tma_load_2d(base + L.codes + cs * Dir::kCtileBytes, &tmap_codes, at.x, at.y + (int)e_rows, cfull_bar(cs));
         }
         __syncwarp();
       };
@@ -358,7 +390,7 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
     const uint4* gcb = reinterpret_cast<const uint4*>(p.codebooks);
     // codebooks of the segment that owns the thread's out row (grouped calls only)
     uint32_t cb_row = 0;
-    if constexpr (GROUPED && !Dir::kRowPerKblock) cb_row = gemm_segment_cb_offset<K>(p, Dir::out_row(pt, m0, 0));
+    if constexpr (GROUPED && !Dir::kRowPerKblock) cb_row = e_cb + gemm_segment_cb_offset<K>(p, Dir::out_row(pt, m0, 0));
     constexpr int CW = (CB4 + 3) / 4;        // 32-bit words holding the thread's CB4 code bytes
     constexpr bool INREG = K <= 2;           // hold the raw gathered vectors in registers until the write
     constexpr int KR = INREG ? K : 1;
@@ -373,9 +405,9 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
       const int kb = kb0 + i;
       const int ct = kb / KB_PER_CTILE, st_in = kb % KB_PER_CTILE;
       const int cs = (ct - ct0) % kCodeTileStages, cit = (ct - ct0) / kCodeTileStages;
-      if constexpr (Dir::kScaleInProducer) sc = Dir::template row_scale<T>(p, pt, kb);
+      if constexpr (Dir::kScaleInProducer) sc = Dir::template row_scale<T>(p, pt, kb, e_rows);
       uint32_t cbo = cb_row;
-      if constexpr (GROUPED && Dir::kRowPerKblock) cbo = gemm_segment_cb_offset<K>(p, Dir::out_row(pt, m0, kb));
+      if constexpr (GROUPED && Dir::kRowPerKblock) cbo = e_cb + gemm_segment_cb_offset<K>(p, Dir::out_row(pt, m0, kb));
       // codebook k's vector `code` (a plain linear: the first and only codebook set)
       auto cb_vec = [&](int k, uint32_t code) -> const uint4* {
         if constexpr (GROUPED) return gcb + (cbo + ((uint32_t)k << p.nbits) + code);
@@ -490,16 +522,22 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
     griddep_wait();
     uint32_t* flag = reinterpret_cast<uint32_t*>(gbase + L.flag);
     const float* parts = p.ws_partials + (tile_id * p.ksplit) * (size_t)N * kGemmBlockM;
-    const int ncols = min(N, p.batch - n0), rows = min(TM, p.m_size - m0);
+    const int ncols = min(N, n_end() - n0), rows = min(TM, p.m_size - m0);
     if constexpr (Dir::kScaleInProducer) {
       gemm_splitk_fixup<T>(flag, p.ws_counters + tile_id, parts, p.ksplit, N, ncols, y, p.m_size, n0, m0, rows, nullptr, nullptr);
     } else {
       if (p.partial_f32)
         gemm_splitk_fixup<T, float>(flag, p.ws_counters + tile_id, parts, p.ksplit, N, ncols, reinterpret_cast<float*>(p.y),
                                     p.m_size, n0, m0, rows, nullptr, nullptr);
-      else
-        gemm_splitk_fixup<T>(flag, p.ws_counters + tile_id, parts, p.ksplit, N, ncols, y, p.m_size, n0, m0, rows,
-                             reinterpret_cast<const T*>(p.scales), reinterpret_cast<const T*>(p.bias));
+      else {
+        const T* scales = reinterpret_cast<const T*>(p.scales);
+        const T* bias = reinterpret_cast<const T*>(p.bias);
+        if constexpr (ROUTED) {
+          scales += e_rows;
+          if (bias) bias += e_rows;
+        }
+        gemm_splitk_fixup<T>(flag, p.ws_counters + tile_id, parts, p.ksplit, N, ncols, y, p.m_size, n0, m0, rows, scales, bias);
+      }
     }
   }
 }
@@ -516,6 +554,14 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_dequant_grouped_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_codes,
                             const GemmParams p) {
   gemm_pipeline<T, N, GemmForward<K, CODE_BYTES>, true>(tmap_x, tmap_codes, p);
+}
+
+// A routed call: every expert of a mixture-of-experts projection in one launch, over expert-sorted input rows.
+template <typename T, int K, int CODE_BYTES, int N>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_dequant_routed_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_codes,
+                           const GemmParams p) {
+  gemm_pipeline<T, N, GemmForward<K, CODE_BYTES>, true, true>(tmap_x, tmap_codes, p);
 }
 
 }  // namespace aqlm_b200

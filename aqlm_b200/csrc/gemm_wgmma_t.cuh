@@ -41,6 +41,8 @@ struct GemmTransposed {
   // The producer multiplies every vector by the scale of its out row; the epilogue and the fix-up only cast.
   static constexpr bool kScaleInProducer = true;
   static __device__ __forceinline__ int tile_m(const GemmParams&) { return kGemmBlockM; }
+  // out rows of one expert of a routed call (the contraction's length)
+  static __device__ __forceinline__ int out_rows(const GemmParams& p) { return p.k_size; }
 
   // code tile: 256 out rows x GBT bytes, un-swizzled; covers 4 k-blocks
   static constexpr int kCtileBytes = kGemmTCtileRows * GBT;
@@ -55,10 +57,11 @@ struct GemmTransposed {
   // the out row of the thread changes with every k-block: a grouped call resolves its segment's codebooks per k-block
   static constexpr bool kRowPerKblock = true;
   static __device__ __forceinline__ int out_row(int pt, int, int kb) { return kb * kGemmBlockK + (pt >> 2); }
+  // e_rows: where a routed call's expert starts in the stacked scales (0 otherwise); o stays relative to the expert
   template <typename T>
-  static __device__ __forceinline__ float row_scale(const GemmParams& p, int pt, int kb) {
+  static __device__ __forceinline__ float row_scale(const GemmParams& p, int pt, int kb, size_t e_rows) {
     const int o = out_row(pt, 0, kb);
-    return o < p.k_size ? DT<T>::to_float(reinterpret_cast<const T*>(p.scales)[o]) : 0.f;  // rows past the end contribute nothing
+    return o < p.k_size ? DT<T>::to_float((reinterpret_cast<const T*>(p.scales) + e_rows)[o]) : 0.f;  // rows past the end contribute nothing
   }
   static __device__ __forceinline__ int code_offset(int pt, int st_in, int q) {
     return (st_in * kGemmBlockK + (pt >> 2)) * GBT + (pt & 3) * CB4 + 16 * q;
@@ -83,6 +86,14 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_dequant_t_grouped_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_constant__ CUtensorMap tmap_codes,
                               const GemmParams p) {
   gemm_pipeline<T, N, GemmTransposed<K, CODE_BYTES>, true>(tmap_g, tmap_codes, p);
+}
+
+// The backward of a routed call: grad_output rows sorted by expert, as the forward's input was.
+template <typename T, int K, int CODE_BYTES, int N>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_dequant_t_routed_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_constant__ CUtensorMap tmap_codes,
+                             const GemmParams p) {
+  gemm_pipeline<T, N, GemmTransposed<K, CODE_BYTES>, true, true>(tmap_g, tmap_codes, p);
 }
 
 }  // namespace aqlm_b200

@@ -257,4 +257,52 @@ inline GemmPlan gemm_t_plan(const aqlm_b200_weight_t& w, int64_t batch, const De
   return g;
 }
 
+// Routed (mixture-of-experts) GEMM over n_experts experts of descriptor w's shape, forward or transposed, `rows` input
+// rows in all.  The routing is on the device, so the plan assumes it balanced: N is the MMA width for ceil(rows / m)
+// rows per expert (m = min(E, rows) experts non-empty), and the tile height and split count are searched over m_tiles x
+// the slots balanced routing keeps busy.  The grid has routed_slot_count() slots, enough for any routing; the slots
+// are the plan's n_tiles (workspace [m_tiles][slots][ksplit][N][128]).  More than kGemmMaxTiles tiles: no split; more
+// slots than a grid dimension holds: no plan.
+inline GemmPlan gemm_routed_plan(const aqlm_b200_weight_t& w, int64_t rows, int n_experts, const DeviceInfo& di,
+                                 const Tunables& t, bool allow_split, bool transposed) {
+  GemmPlan g;
+  const int K = w.num_codebooks, nbits = w.nbits_per_codebook;
+  const int cb = nbits <= 8 ? 1 : 2;
+  if (rows < 1 || n_experts < 1 || !gemm_scheme_ok(w, t)) return g;
+  if (transposed ? (16 * K * cb > 256 || w.out_features % 8 != 0)
+                 : (8 * K * cb > kCodeTileBytes || w.in_features % kGemmBlockK != 0))
+    return g;
+  const int64_t m = rows < n_experts ? rows : n_experts;
+  int per_expert_tiles = 0;
+  gemm_n_tiles((rows + m - 1) / m, &g.n_tile, &per_expert_tiles);
+  const long long slots = routed_slot_count(rows, n_experts, g.n_tile);
+  if (slots > 65535) return g;
+  g.n_tiles = (int)slots;
+  const long long active = m * (long long)per_expert_tiles;
+  const int ctile_bytes = transposed ? kGemmTCtileRows * 16 * K * cb : kGemmBlockM * kCodeTileBytes;
+  g.stages = gemm_stages([&](int s) { return gemm_smem_layout(s, g.n_tile, ctile_bytes).total; },
+                         (size_t)di.max_smem_optin, t.gemm_stages, transposed ? 3 : 4);
+  if (!g.stages) return g;
+  g.total_kblocks = (int)(transposed ? (w.out_features + kGemmBlockK - 1) / kGemmBlockK : w.in_features / kGemmBlockK);
+  const int max_ks = allow_split ? gemm_max_ksplit(g.total_kblocks) : 1;
+  int best_tm = kGemmBlockM, best_ks = 1;
+  double best = 1e30;
+  if (transposed) {
+    gemm_split_search(kGemmBlockM, ((w.in_features + kGemmBlockM - 1) / kGemmBlockM) * active, K, nbits, g.n_tile,
+                      g.total_kblocks, max_ks, di.sm_count, &best, &best_tm, &best_ks);
+  } else {
+    for (int tm = kGemmBlockM; tm >= 32; tm -= (tm > 64 ? 1 : 8)) {
+      const long long tiles = ((w.out_features + tm - 1) / tm) * active;
+      if (tiles > kGemmMaxTiles) continue;
+      gemm_split_search(tm, tiles, K, nbits, g.n_tile, g.total_kblocks, max_ks, di.sm_count, &best, &best_tm, &best_ks);
+    }
+    g.tile_m = best_tm;
+    if (t.gemm_tile_m >= 8 && t.gemm_tile_m <= kGemmBlockM) g.tile_m = t.gemm_tile_m;
+  }
+  const int64_t m_size = transposed ? w.in_features : w.out_features;
+  g.m_tiles = (int)((m_size + g.tile_m - 1) / g.tile_m);
+  gemm_finish(g, best_ks, allow_split, t);  // more than kGemmMaxTiles tiles (m_tiles x slots): no split
+  return g;
+}
+
 }  // namespace aqlm_b200

@@ -11,6 +11,13 @@ grouped launches wired into a loaded model.
   q/k/v, MLP gate/up) and makes each set run as ONE grouped launch (`QuantizedLinearGroup`: the grouped GEMV at decode,
   the grouped GEMM at prefill and in training), without changing module names, the state dict, or the model's forward
   code: the members' `forward` is routed through a small per-group cache.
+* `load_quantized_mixtral` loads an AQLM Mixtral checkpoint (e.g. `ISTA-DASLab/Mixtral-8x7b-AQLM-2Bit-1x16-hf`) with
+  quantized experts.  `from_pretrained` alone cannot: in transformers 5.x a Mixtral block keeps all its experts as two
+  dense 3-D parameters (`MixtralExperts.gate_up_proj` / `down_proj`), Hugging Face's AQLM integration replaces
+  `nn.Linear` modules only, so the experts stay dense placeholders (about 90 GB of fp16 for Mixtral-8x7B) and the
+  checkpoint's per-expert tensors `block_sparse_moe.experts.{e}.w{1,2,3}.{codes,codebooks,scales}` have nowhere to
+  load.  `replace_mixtral_experts` swaps every block's experts for `moe.QuantizedMixtralExperts` (one routed GEMM per
+  projection over all experts), whose state-dict names are the checkpoint's.
 """
 from __future__ import annotations
 
@@ -24,6 +31,7 @@ from torch import nn
 
 from .grouped import QuantizedLinearGroup, _rows, gemm_scheme
 from .inference import QuantizedLinear
+from .moe import QuantizedMixtralExperts
 from .utils import pack_int_data
 
 #: attribute-name sets of linears that share their input, per parent module (Llama / Mistral / Qwen2 / Gemma layouts)
@@ -133,3 +141,86 @@ def save_quantized_checkpoint(save_dir: str, config_dict: Dict, state_dict: Dict
     except ImportError:
         torch.save(tensors, os.path.join(save_dir, "pytorch_model.bin"))
     return save_dir
+
+
+def _aqlm_config(model: nn.Module) -> Dict:
+    qc = getattr(model.config, "quantization_config", None)
+    if qc is None:
+        raise ValueError("the model's config has no quantization_config (not an AQLM checkpoint)")
+    return qc if isinstance(qc, dict) else qc.to_dict()
+
+
+def replace_mixtral_experts(model: nn.Module) -> int:
+    """Swap the experts of every `MixtralSparseMoeBlock` of `model` for `QuantizedMixtralExperts` with the model's AQLM
+    scheme, on the device (meta included) and in the dtype of the block's router.  Returns the number of blocks."""
+    from transformers.models.mixtral.modeling_mixtral import MixtralSparseMoeBlock
+
+    qc = _aqlm_config(model)
+    n = 0
+    for block in model.modules():
+        if not isinstance(block, MixtralSparseMoeBlock) or isinstance(block.experts, QuantizedMixtralExperts):
+            continue
+        old, w = block.experts, block.gate.weight
+        block.experts = QuantizedMixtralExperts(
+            old.num_experts, old.hidden_dim, old.intermediate_dim, old.act_fn, in_group_size=qc["in_group_size"],
+            out_group_size=qc["out_group_size"], num_codebooks=qc["num_codebooks"],
+            nbits_per_codebook=qc["nbits_per_codebook"], device=w.device, dtype=w.dtype)
+        n += 1
+    return n
+
+
+def _checkpoint_state_dict(path: str) -> Dict[str, torch.Tensor]:
+    """Every tensor of the checkpoint directory (safetensors shards, else `.bin` shards), by name."""
+    files = sorted(f for f in os.listdir(path) if f.endswith(".safetensors"))
+    sd: Dict[str, torch.Tensor] = {}
+    if files:
+        from safetensors.torch import load_file
+
+        for f in files:
+            sd.update(load_file(os.path.join(path, f)))
+        return sd
+    for f in sorted(f for f in os.listdir(path) if f.endswith(".bin")):
+        sd.update(torch.load(os.path.join(path, f), map_location="cpu", weights_only=True))
+    if not sd:
+        raise FileNotFoundError(f"no .safetensors or .bin weights in {path}")
+    return sd
+
+
+def load_quantized_mixtral(path: str, dtype: torch.dtype = torch.float16, device="cuda") -> nn.Module:
+    """Load an AQLM Mixtral checkpoint directory with quantized experts (see the module docstring for why
+    `from_pretrained` does not).  The model is built on the meta device, Hugging Face's `replace_with_aqlm_linear` makes
+    the attention projections `QuantizedLinear`s (ours, through `install_as_aqlm`), `replace_mixtral_experts` the
+    experts; the weights are loaded by name (`.block_sparse_moe.` renamed to `.mlp.`, as transformers does) strictly,
+    then the model moves to `device`.  No dense expert tensor is ever allocated."""
+    from transformers import AutoConfig, AutoModelForCausalLM
+    from transformers.integrations.aqlm import replace_with_aqlm_linear
+    from transformers.utils.quantization_config import AqlmConfig
+
+    from . import install_as_aqlm
+
+    install_as_aqlm()  # replace_with_aqlm_linear builds `aqlm.QuantizedLinear`
+    config = AutoConfig.from_pretrained(path)
+    with torch.device("meta"):
+        model = AutoModelForCausalLM.from_config(config, dtype=dtype)
+    qc = _aqlm_config(model)
+    # the reference converter lists PARAMETER names (`lm_head.weight`); transformers >= 5 matches MODULE names
+    keep = list(qc.get("linear_weights_not_to_quantize") or [])
+    keep += [n[: -len(".weight")] for n in keep if n.endswith(".weight")]
+    replace_with_aqlm_linear(model, modules_to_not_convert=keep, quantization_config=AqlmConfig.from_dict(qc))
+    replace_mixtral_experts(model)
+    sd = {k.replace(".block_sparse_moe.", ".mlp."): v for k, v in _checkpoint_state_dict(path).items()}
+    sd = {k: (v.to(dtype) if v.is_floating_point() else v) for k, v in sd.items()}
+    if getattr(config, "tie_word_embeddings", False) and "lm_head.weight" not in sd:
+        sd["lm_head.weight"] = sd["model.embed_tokens.weight"]
+    model.load_state_dict(sd, strict=True, assign=True)
+    if getattr(config, "tie_word_embeddings", False):
+        model.tie_weights()
+    for m in model.modules():
+        if isinstance(m, QuantizedMixtralExperts):
+            m.fuse_storage()  # the load replaced the members' parameters
+    # modules with buffers that are not in the checkpoint (the rotary embedding's inverse frequencies) still hold meta
+    # tensors: build them again for real
+    for name, mod in list(model.named_modules()):
+        if any(b.is_meta for b in mod.buffers(recurse=False)):
+            model.set_submodule(name, type(mod)(mod.config, device="cpu"))
+    return model.to(device).eval()

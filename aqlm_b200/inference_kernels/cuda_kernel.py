@@ -283,6 +283,89 @@ def matmat_dequant_transposed_grouped(grad_out, codes, codebooks_stacked, scales
     return out.reshape(grad_out.shape[:-1] + (w.in_features,))
 
 
+def _routed_weight(codes, codebooks_stacked, scales, seg_rows):
+    """Descriptor of ONE expert whose pointers point at the stacks of all experts: codes [E, out, in/8, K], codebooks
+    [E, n_seg, K, 2^nbits, 1, 8], scales [E, out, ...]."""
+    n_experts, n_seg = codebooks_stacked.shape[:2]
+    if codes.dim() != 4 or codes.shape[0] != n_experts or codebooks_stacked.dim() != 6:
+        raise ValueError("routed GEMM takes codes [E, out, in/8, K] and codebooks [E, n_seg, K, 2^nbits, 1, 8]")
+    if not codebooks_stacked.is_contiguous() or (seg_rows is not None and len(seg_rows) != n_seg):
+        raise ValueError("codebooks must be a contiguous [E, n_seg, ...] stack matching seg_rows")
+    if scales.numel() != codes.shape[0] * codes.shape[1]:
+        raise ValueError(f"scales have {scales.numel()} elements for {codes.shape[0]} experts of {codes.shape[1]} rows")
+    w = make_weight(codes[0], codebooks_stacked[0, 0], scales.reshape(-1), None)
+    seg = None if seg_rows is None else (ctypes.c_int64 * n_seg)(*[int(r) for r in seg_rows])
+    return w, seg, (n_seg if seg_rows is not None else 1), n_experts
+
+
+def _check_offsets(expert_offsets, n_experts, device):
+    if expert_offsets.dtype != torch.int32 or expert_offsets.numel() != n_experts + 1 or \
+            expert_offsets.device != device or not expert_offsets.is_contiguous():
+        raise ValueError(f"expert_offsets must be a contiguous int32 tensor of {n_experts + 1} elements on {device}")
+
+
+def matmat_dequant_routed(input, codes, codebooks_stacked, scales, expert_offsets, seg_rows=None) -> Optional[torch.Tensor]:
+    """ONE wgmma GEMM launch for every expert of a mixture-of-experts projection: row r of `input` [rows, in] (sorted by
+    expert) is multiplied by the weight of the expert e with expert_offsets[e] <= r < expert_offsets[e + 1].  `codes`
+    [E, out, in/8, K], `codebooks_stacked` [E, n_seg, K, 2^nbits, 1, 8] (`seg_rows`: the out rows of each of an expert's
+    n_seg row-concatenated linears, None for one), `scales` [E, out, ...], `expert_offsets` int32 [E + 1] on the device
+    (never read by the host: the call is graph-capturable).  Returns [rows, out] in the input dtype; rows outside
+    [offsets[0], offsets[E]) are left unwritten.  Returns None when the library does not take the layout."""
+    device = _require_cuda(input, codes, codebooks_stacked, scales, expert_offsets)
+    _dtype_code(input)
+    if input.dtype != codebooks_stacked.dtype:
+        raise ValueError(f"input dtype {input.dtype} != codebooks dtype {codebooks_stacked.dtype}")
+    w, seg, n_seg, n_experts = _routed_weight(codes, codebooks_stacked, scales, seg_rows)
+    _check_offsets(expert_offsets, n_experts, device)
+    if input.dim() != 2 or input.shape[-1] != w.in_features:
+        raise ValueError(f"input must be [rows, {w.in_features}], got {tuple(input.shape)}")
+    flat = input if input.is_contiguous() else input.contiguous()
+    rows = flat.shape[0]
+    out = torch.empty((rows, w.out_features), dtype=input.dtype, device=device)
+    with _on_device(device):
+        L = _cabi.lib()
+        need = L.aqlm_b200_matmat_dequant_routed_workspace_bytes(ctypes.byref(w), n_experts, rows, 0) if rows else 0
+        ws = _workspace(device, need) if need else None
+        rc = L.aqlm_b200_matmat_dequant_routed(ctypes.byref(w), seg, n_seg, n_experts, expert_offsets.data_ptr(),
+                                               flat.data_ptr(), out.data_ptr(), rows,
+                                               ws.data_ptr() if ws is not None else None,
+                                               ws.numel() if ws is not None else 0, _stream_ptr(device))
+    if rc == _cabi.ERR_UNSUPPORTED:
+        return None
+    _cabi.check(rc)
+    return out
+
+
+def matmat_dequant_transposed_routed(grad_out, codes, codebooks_stacked, scales, expert_offsets,
+                                     seg_rows=None) -> Optional[torch.Tensor]:
+    """Backward w.r.t. the input of `matmat_dequant_routed` in ONE transposed wgmma GEMM launch: row r of grad_input is
+    (grad_out[r] * scales_e) @ W_e for the expert e that owns row r.  Same arguments; rows outside [offsets[0],
+    offsets[E]) are left unwritten.  Returns None when the library does not take the layout."""
+    device = _require_cuda(grad_out, codes, codebooks_stacked, scales, expert_offsets)
+    _dtype_code(grad_out)
+    if grad_out.dtype != codebooks_stacked.dtype:
+        raise ValueError(f"grad_output dtype {grad_out.dtype} != codebooks dtype {codebooks_stacked.dtype}")
+    w, seg, n_seg, n_experts = _routed_weight(codes, codebooks_stacked, scales, seg_rows)
+    _check_offsets(expert_offsets, n_experts, device)
+    if grad_out.dim() != 2 or grad_out.shape[-1] != w.out_features:
+        raise ValueError(f"grad_output must be [rows, {w.out_features}], got {tuple(grad_out.shape)}")
+    flat = grad_out if grad_out.is_contiguous() else grad_out.contiguous()
+    rows = flat.shape[0]
+    out = torch.empty((rows, w.in_features), dtype=grad_out.dtype, device=device)
+    with _on_device(device):
+        L = _cabi.lib()
+        need = L.aqlm_b200_matmat_dequant_routed_workspace_bytes(ctypes.byref(w), n_experts, rows, 1) if rows else 0
+        ws = _workspace(device, need) if need else None
+        rc = L.aqlm_b200_matmat_dequant_transposed_routed(ctypes.byref(w), seg, n_seg, n_experts,
+                                                          expert_offsets.data_ptr(), flat.data_ptr(), out.data_ptr(),
+                                                          rows, ws.data_ptr() if ws is not None else None,
+                                                          ws.numel() if ws is not None else 0, _stream_ptr(device))
+    if rc == _cabi.ERR_UNSUPPORTED:
+        return None
+    _cabi.check(rc)
+    return out
+
+
 def matmat_partial(input, codes, codebooks) -> torch.Tensor:
     """UNSCALED fp32 partial products [batch, out] of an in_features shard (to be all-reduced).  Above GEMV_MAX_ROWS
     rows (prefill) this is the wgmma GEMM, as in QuantizedLinear; below, the GEMV / LUT kernels."""

@@ -147,6 +147,33 @@ int aqlm_b200_matmat_dequant_transposed_grouped(const aqlm_b200_weight_t* w, con
                                                 const void* grad_output, void* grad_input, int64_t batch, void* workspace,
                                                 size_t workspace_bytes, void* stream);
 
+/* Routed form of the two tensor-core GEMMs, for a mixture-of-experts projection: n_experts experts of one shape in ONE
+ * launch, each applied to its own run of rows.  `w` describes ONE expert (out_features = sum(seg_rows)), and its
+ * pointers point at the stacks of all experts: codes [E][out][in/8][K], codebooks [E][n_seg][K][2^nbits][8], scales and
+ * bias [E][out].  `seg_rows` / `n_seg` split each expert's rows as for the grouped GEMM (Mixtral's w1|w3 pair: n_seg 2);
+ * seg_rows == NULL with n_seg == 1 is a plain expert linear.
+ *   forward:     output[r] = input[r] . W_e^T * scales_e + bias_e  for the expert e that owns row r;
+ *                input [rows, in], output [rows, out]
+ *   transposed:  grad_input[r] = (grad_output[r] * scales_e) . W_e;  grad_output [rows, out], grad_input [rows, in]
+ * `expert_offsets` is a DEVICE int32 array [n_experts + 1]: expert e owns rows [off[e], off[e+1]), so the rows must be
+ * sorted by expert.  The host never reads it: the call is capturable in a CUDA graph, and the routing may change between
+ * replays.  The offsets are not trusted: each is clamped into [0, rows] and raised to its predecessor (a decreasing pair
+ * is an empty expert), and rows outside [off[0], off[E]) are neither read for output nor written (their output rows keep
+ * whatever they held).  The workspace (split-K) comes from aqlm_b200_matmat_dequant_routed_workspace_bytes; without it
+ * the call runs unsplit.  Errors, before any device query: AQLM_B200_ERR_SHAPE for a bad descriptor, n_seg outside 1..4,
+ * segments that do not add up to out_features, n_experts outside 1..64, or NULL offsets / buffers;
+ * AQLM_B200_ERR_UNSUPPORTED for layouts the wgmma kernels do not take (as for the grouped GEMM).  rows == 0: OK, no
+ * launch.  Exactly one launch otherwise. */
+size_t aqlm_b200_matmat_dequant_routed_workspace_bytes(const aqlm_b200_weight_t* w, int n_experts, int64_t rows,
+                                                       int transposed);
+int aqlm_b200_matmat_dequant_routed(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, int n_experts,
+                                    const int32_t* expert_offsets, const void* input, void* output, int64_t rows,
+                                    void* workspace, size_t workspace_bytes, void* stream);
+int aqlm_b200_matmat_dequant_transposed_routed(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg,
+                                               int n_experts, const int32_t* expert_offsets, const void* grad_output,
+                                               void* grad_input, int64_t rows, void* workspace, size_t workspace_bytes,
+                                               void* stream);
+
 /* Epilogue of the sharded path: output[b,o] = (T)(partial[b,o] * scales[o] + bias[o]) after the
  * all-reduce of the fp32 partials (new work; the reference has no multi-GPU hot path, SURVEY §8e). */
 int aqlm_b200_scale_bias(const float* partial, const void* scales, const void* bias, void* output, int64_t batch,
