@@ -694,6 +694,58 @@ static int routed_gemm(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int
   });
 }
 
+// ---- fused weight-gradient GEMM: host side ------------------------------------------------------------------------
+// Everything a weight-gradient call checks without a device: descriptor, pointers (ERR_SHAPE), then the layouts the
+// kernel takes (ERR_UNSUPPORTED).
+static int weight_grad_checks(const aqlm_b200_weight_t* w, const void* input, const void* grad_output, int64_t batch,
+                              const float* grad_codebooks, const float* grad_scales) {
+  int rc = validate(w, grad_codebooks != nullptr);
+  if (rc) return rc;
+  if (batch < 0 || batch > 0x7fffffffll) return fail(AQLM_B200_ERR_SHAPE, "weight gradient: batch %lld out of range", (long long)batch);
+  if (!input || !grad_output) return fail(AQLM_B200_ERR_SHAPE, "weight gradient: input/grad_output pointer is NULL");
+  if (!grad_codebooks && !grad_scales)
+    return fail(AQLM_B200_ERR_SHAPE, "weight gradient: neither grad_codebooks nor grad_scales requested");
+  const int K = w->num_codebooks, nbits = w->nbits_per_codebook, cb = nbits <= 8 ? 1 : 2;
+  if (w->in_group_size != 8 || (nbits != 8 && nbits != 16) || !(K == 1 || K == 2 || K == 4 || K == 8))
+    return fail(AQLM_B200_ERR_UNSUPPORTED,
+                "weight gradient covers in_group_size 8, 8/16-bit codes and 1/2/4/8 codebooks; got %dx%d, in_group_size %d",
+                K, nbits, w->in_group_size);
+  if (w->out_features % 8 != 0)
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "weight gradient needs out_features %% 8 == 0, got %lld", (long long)w->out_features);
+  if (((size_t)(w->in_features / 8) * K * cb) % 16 != 0 || (reinterpret_cast<uintptr_t>(w->codes) & 15) != 0)
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "weight gradient needs 16-byte aligned code rows");
+  if ((reinterpret_cast<uintptr_t>(input) & 15) != 0 || (reinterpret_cast<uintptr_t>(grad_output) & 15) != 0)
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "weight gradient needs a 16-byte aligned input and grad_output");
+  return AQLM_B200_OK;
+}
+
+template <typename T, int K, int CB>
+static int launch_weight_grad(const aqlm_b200_weight_t* w, const void* input, const void* grad_output, int64_t batch,
+                              float* grad_codebooks, float* grad_scales, void* workspace, const WgradPlan& g,
+                              const DeviceInfo* di, cudaStream_t st) {
+  CUtensorMap tg, tx;
+  if (int rc = encode_tmap(&tg, "grad_output", kTmapType<T>, grad_output, w->out_features, batch, w->out_features * 2, 64,
+                           kWgradBlockK, CU_TENSOR_MAP_SWIZZLE_128B))
+    return rc;
+  if (int rc = encode_tmap(&tx, "input", kTmapType<T>, input, w->in_features, batch, w->in_features * 2, 64, kWgradBlockK,
+                           CU_TENSOR_MAP_SWIZZLE_128B))
+    return rc;
+  WgradParams p;
+  p.codes = w->codes;
+  p.codebooks = w->codebooks;
+  p.scales = w->scales;
+  p.grad_codebooks = grad_codebooks;
+  p.grad_scales = grad_scales;
+  p.ws_counters = grad_scales ? reinterpret_cast<unsigned int*>(workspace) : nullptr;
+  p.ws_dots = grad_scales ? reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + g.counters_bytes) : nullptr;
+  p.out_features = (int)w->out_features;
+  p.in_features = (int)w->in_features;
+  p.nbits = w->nbits_per_codebook;
+  p.total_kblocks = g.total_kblocks;
+  p.stages = g.stages;
+  return launch<gemm_wgrad_kernel<T, K, CB>>(di, dim3(g.out_tiles, g.in_tiles), kWgradThreads, g.smem, st, 0, tg, tx, p);
+}
+
 }  // namespace aqlm_b200
 
 using namespace aqlm_b200;
@@ -944,6 +996,35 @@ int aqlm_b200_matmat_dequant_transposed_routed(const aqlm_b200_weight_t* w, cons
                                                void* stream) {
   return routed_gemm<true>(w, seg_rows, n_seg, n_experts, expert_offsets, grad_output, grad_input, rows, workspace,
                            workspace_bytes, stream);
+}
+
+size_t aqlm_b200_matmat_weight_grad_workspace_bytes(const aqlm_b200_weight_t* w, int64_t batch) {
+  if (validate(w, false) != AQLM_B200_OK || batch <= 0) return 0;
+  const DeviceInfo* di = device_info();
+  if (!di) return 0;
+  const WgradPlan g = gemm_wgrad_plan(*w, batch, *di, tun());
+  return g.ok ? g.counters_bytes + g.dots_bytes : 0;
+}
+
+int aqlm_b200_matmat_weight_grad(const aqlm_b200_weight_t* w, const void* input, const void* grad_output,
+                                 int64_t batch, float* grad_codebooks, float* grad_scales, void* workspace,
+                                 size_t workspace_bytes, void* stream) {
+  int rc = weight_grad_checks(w, input, grad_output, batch, grad_codebooks, grad_scales);
+  if (rc || batch == 0) return rc;
+  const DeviceInfo* di;
+  if ((rc = current_device(&di))) return rc;
+  const WgradPlan g = gemm_wgrad_plan(*w, batch, *di, tun());
+  if (!g.ok) return fail(AQLM_B200_ERR_UNSUPPORTED, "weight gradient: no wgmma plan for this descriptor and batch");
+  if (grad_scales && (!workspace || workspace_bytes < g.counters_bytes + g.dots_bytes))
+    return fail(AQLM_B200_ERR_SHAPE, "weight gradient: grad_scales needs a workspace of %zu bytes, got %zu",
+                g.counters_bytes + g.dots_bytes, workspace ? workspace_bytes : (size_t)0);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return with_dtype(w->dtype, [&](auto tag) {
+    return with_gemm_scheme(w, [&](auto K, auto CB) {
+      return launch_weight_grad<typename decltype(tag)::type, K, CB>(w, input, grad_output, batch, grad_codebooks,
+                                                                     grad_scales, workspace, g, di, st);
+    });
+  });
 }
 
 int aqlm_b200_scale_bias(const float* partial, const void* scales, const void* bias, void* output, int64_t batch,

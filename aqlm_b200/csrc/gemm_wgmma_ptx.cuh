@@ -57,7 +57,7 @@ __device__ __forceinline__ void acc_fence(float (&d)[R]) {
 
 // One wgmma.mma_async m64nNk16 statement per width, over the names d, a, b, TA of wgmma_tile below; TY is the
 // instruction's operand type token ("f16" or "bf16"), the only thing the two data types differ in.  N / 2 accumulator
-// registers, then the A and B descriptors, the scale-d predicate and the transpose-A immediate.
+// registers, then the A and B descriptors, the scale-d predicate and the transpose-A and transpose-B immediates.
 #define AQLM_WGMMA_D8(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
 #define AQLM_WGMMA_D16(o) AQLM_WGMMA_D8(o), AQLM_WGMMA_D8(o + 8)
 #define AQLM_WGMMA_D32(o) AQLM_WGMMA_D16(o), AQLM_WGMMA_D16(o + 16)
@@ -66,25 +66,26 @@ __device__ __forceinline__ void acc_fence(float (&d)[R]) {
 #define AQLM_WGMMA_R16 ", %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
 #define AQLM_WGMMA_R32 ", %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
 #define AQLM_WGMMA_R48 ", %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
-// SHAPE "m64nNk16"; DREGS the accumulator placeholders; A, B, P, TAI the placeholders that follow them
-#define AQLM_WGMMA(SHAPE, TY, DREGS, A, B, P, TAI, ...)                                   \
+// SHAPE "m64nNk16"; DREGS the accumulator placeholders; A, B, P, TAI, TBI the placeholders that follow them
+#define AQLM_WGMMA(SHAPE, TY, DREGS, A, B, P, TAI, TBI, ...)                              \
   asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, " P ", 0;\n"                              \
                "wgmma.mma_async.sync.aligned." SHAPE ".f32." TY "." TY " "                 \
-               "{" DREGS "}, " A ", " B ", p, 1, 1, " TAI ", 0;\n}\n"                      \
+               "{" DREGS "}, " A ", " B ", p, 1, 1, " TAI ", " TBI ";\n}\n"                \
                : __VA_ARGS__                                                               \
-               : "l"(a), "l"(b), "r"(1), "n"(TA))
-#define AQLM_WGMMA_N16(TY) AQLM_WGMMA("m64n16k16", TY, AQLM_WGMMA_R0, "%8", "%9", "%10", "%11", AQLM_WGMMA_D8(0))
+               : "l"(a), "l"(b), "r"(1), "n"(TA), "n"(TB))
+#define AQLM_WGMMA_N16(TY) AQLM_WGMMA("m64n16k16", TY, AQLM_WGMMA_R0, "%8", "%9", "%10", "%11", "%12", AQLM_WGMMA_D8(0))
 #define AQLM_WGMMA_N32(TY) \
-  AQLM_WGMMA("m64n32k16", TY, AQLM_WGMMA_R0 AQLM_WGMMA_R8, "%16", "%17", "%18", "%19", AQLM_WGMMA_D16(0))
-#define AQLM_WGMMA_N64(TY) \
-  AQLM_WGMMA("m64n64k16", TY, AQLM_WGMMA_R0 AQLM_WGMMA_R8 AQLM_WGMMA_R16, "%32", "%33", "%34", "%35", AQLM_WGMMA_D32(0))
+  AQLM_WGMMA("m64n32k16", TY, AQLM_WGMMA_R0 AQLM_WGMMA_R8, "%16", "%17", "%18", "%19", "%20", AQLM_WGMMA_D16(0))
+#define AQLM_WGMMA_N64(TY)                                                                                             \
+  AQLM_WGMMA("m64n64k16", TY, AQLM_WGMMA_R0 AQLM_WGMMA_R8 AQLM_WGMMA_R16, "%32", "%33", "%34", "%35", "%36", \
+             AQLM_WGMMA_D32(0))
 #define AQLM_WGMMA_N128(TY)                                                                                          \
   AQLM_WGMMA("m64n128k16", TY, AQLM_WGMMA_R0 AQLM_WGMMA_R8 AQLM_WGMMA_R16 AQLM_WGMMA_R32 AQLM_WGMMA_R48, "%64", "%65", \
-             "%66", "%67", AQLM_WGMMA_D32(0), AQLM_WGMMA_D32(32))
+             "%66", "%67", "%68", AQLM_WGMMA_D32(0), AQLM_WGMMA_D32(32))
 
-// D[64 x N] += A[64 x 16] . B[N x 16]^T in T (fp16 or bf16), fp32 accumulate; TA = 1: A is MN-major (transposed), B is
-// K-major
-template <typename T, int N, int TA>
+// D[64 x N] += A[64 x 16] . B[N x 16]^T in T (fp16 or bf16), fp32 accumulate; TA = 1: A is MN-major (transposed);
+// TB = 1: B is MN-major (transposed); 0: K-major
+template <typename T, int N, int TA, int TB = 0>
 __device__ __forceinline__ void wgmma_tile(float* d, uint64_t a, uint64_t b) {
   static_assert(N == 16 || N == 32 || N == 64 || N == 128, "wgmma tile width");
   if constexpr (DT<T>::is_bf16) {

@@ -8,6 +8,7 @@
 #include "common.cuh"
 #include "gemm_wgmma.cuh"
 #include "gemm_wgmma_t.cuh"
+#include "gemm_wgrad.cuh"
 #include "gemv.cuh"
 #include "gemv_lut.cuh"
 
@@ -302,6 +303,37 @@ inline GemmPlan gemm_routed_plan(const aqlm_b200_weight_t& w, int64_t rows, int 
   const int64_t m_size = transposed ? w.in_features : w.out_features;
   g.m_tiles = (int)((m_size + g.tile_m - 1) / g.tile_m);
   gemm_finish(g, best_ks, allow_split, t);  // more than kGemmMaxTiles tiles (m_tiles x slots): no split
+  return g;
+}
+
+// ---- fused weight-gradient GEMM (gradients of codebooks and scales) -------------------------------------------------
+struct WgradPlan {
+  bool ok = false;
+  int out_tiles = 0, in_tiles = 0, stages = 0, total_kblocks = 0;
+  size_t smem = 0, counters_bytes = 0, dots_bytes = 0;  // workspace: counters, then [in_tiles][out] fp32 row dots
+};
+
+// grad_codebooks / grad_scales from input [batch][in] and grad_output [batch][out]: one CTA per 128 x 128 tile of
+// D = grad_output^T input, the batch is the contraction.  The schemes of gemm_scheme_ok, and out % 8 == 0 (TMA row
+// stride of grad_output).  Stages as the forward's (at most 4 when forced); the epilogue's memory (the staged D, 64 KiB +
+// padding, and for 8-bit codes the CTA's K x 256 x 8 fp32 codebook gradient) reuses the pipeline's.
+inline WgradPlan gemm_wgrad_plan(const aqlm_b200_weight_t& w, int64_t batch, const DeviceInfo& di, const Tunables& t) {
+  WgradPlan g;
+  if (batch < 1 || !gemm_scheme_ok(w, t) || w.out_features % 8 != 0) return g;
+  const int64_t out_tiles = (w.out_features + kWgradTile - 1) / kWgradTile;
+  const int64_t in_tiles = (w.in_features + kWgradTile - 1) / kWgradTile;
+  if (out_tiles > kGemmMaxTiles || in_tiles > 65535) return g;  // one ticket word per out tile; grid.y
+  g.out_tiles = (int)out_tiles;
+  g.in_tiles = (int)in_tiles;
+  g.total_kblocks = (int)((batch + kWgradBlockK - 1) / kWgradBlockK);
+  const int cb_bytes = wgrad_cb_smem_bytes(w.num_codebooks, w.nbits_per_codebook);
+  g.stages = gemm_stages([&](int s) { return gemm_wgrad_smem_layout(s, cb_bytes).total; }, (size_t)di.max_smem_optin,
+                         t.gemm_stages, 4);
+  if (!g.stages) return g;
+  g.smem = gemm_wgrad_smem_layout(g.stages, cb_bytes).total;
+  g.counters_bytes = kWsCountersBytes;
+  g.dots_bytes = (size_t)g.in_tiles * w.out_features * 4;
+  g.ok = true;
   return g;
 }
 

@@ -10,7 +10,8 @@ Which launch serves a call:
   * more rows, or an input that needs a gradient, for every scheme the wgmma GEMM covers (in_group 8, 8/16-bit codes,
     1/2/4/8 codebooks): the grouped GEMM over the row-concatenated weight (one launch), and for the gradient w.r.t. the
     input one grouped transposed GEMM (`_GroupedMatmul`);
-  * anything else -- up to 8 rows of other schemes, or a layout the library refuses -- the members one by one.
+  * anything else -- up to 8 rows of other schemes, or a layout the library refuses -- the members one by one;
+  * so do calls that need a gradient w.r.t. a member's codebooks, scales or bias (no grouped weight-gradient kernel).
 """
 from __future__ import annotations
 
@@ -19,7 +20,7 @@ from typing import Sequence, Tuple
 import torch
 import torch.nn as nn
 
-from .inference import QuantizedLinear
+from .inference import QuantizedLinear, weights_require_grad
 from .sharded import ShardedQuantizedLinear
 
 
@@ -124,6 +125,10 @@ class QuantizedLinearGroup(nn.Module):
         needs_grad = torch.is_grad_enabled() and input.requires_grad
         if not self.fused or not input.is_cuda or rows < 1:
             return tuple(m(input) for m in self.members)
+        if torch.is_grad_enabled() and any(weights_require_grad(m) for m in self.members):
+            # trainable codebooks / scales / bias: each member's own autograd node computes its weight gradients, which
+            # land on the member parameters (views into the fused storage)
+            return tuple(m(input) for m in self.members)
         from .inference_kernels import cuda_kernel
 
         if rows <= 8 and _gemv_scheme(self.members[0]):
@@ -168,6 +173,8 @@ class ShardedQuantizedLinearGroup(nn.Module):
                 self._fused_bias = None
 
     def forward(self, input: torch.Tensor) -> Tuple[torch.Tensor, ...]:
+        if torch.is_grad_enabled() and any(weights_require_grad(m) for m in self.members):
+            raise NotImplementedError("the sharded path has no weight gradient: freeze codebooks, scales and bias")
         local = self.in_end - self.in_begin
         if input.shape[-1] == self.in_features and self.world_size > 1:
             input = input[..., self.in_begin:self.in_end]

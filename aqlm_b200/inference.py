@@ -7,7 +7,7 @@ integration and existing checkpoints depend on it:
   * frozen parameters `codebooks [K, 2^nbits, og, ig]`, `codes [out/og, in/ig, K]` (signed storage of unsigned codes),
     `scales [out/og, 1, 1, 1]`, optional `bias [out]` (inference.py:39-61) -- the state_dict names / shapes / dtypes;
   * small inputs (<= 6 rows, inference.py:95-96) go to the fused GEMV op, larger ones to the fused dequant + tensor-core
-    GEMM op; gradients flow to the input only (inference.py:99-142).
+    GEMM op; gradients flow to the input (inference.py:99-142) and, once unfrozen, to codebooks, scales and bias.
 What differs: no CPU path (CPU inputs raise), no in-place re-layout of `codes` on first use (inference.py:78-83), no JIT
 build on first call -- the ops are bound once and cached.
 """
@@ -27,19 +27,36 @@ GEMV_MAX_ROWS = 6
 
 
 class _AqlmMatmul(torch.autograd.Function):
-    """y = op(x; codes, codebooks, scales, bias).  Only `x` receives a gradient; the quantized weight is frozen."""
+    """y = op(x; codes, codebooks, scales, bias).  Gradients reach x and whichever of codebooks, scales and bias require
+    them; `codes` are integers and get none.  The codebook and scale gradients come from ONE fused weight-gradient GEMM
+    (`cuda_kernel.matmat_weight_grad`), for which x is saved; the bias gradient is grad_y summed over rows in fp32."""
 
     @staticmethod
     def forward(ctx, x, codes, codebooks, scales, bias, forward_op: Callable, backward_op: Callable):
         ctx.backward_op = backward_op
-        ctx.save_for_backward(codes, codebooks, scales, bias)
+        wgrad = ctx.needs_input_grad[2] or ctx.needs_input_grad[3]
+        ctx.save_for_backward(codes, codebooks, scales, bias, x if wgrad else None)
         return forward_op(x, codes, codebooks, scales, bias)
 
     @staticmethod
     def backward(ctx, grad_y):
-        codes, codebooks, scales, bias = ctx.saved_tensors
-        grad_x = ctx.backward_op(grad_y, codes, codebooks, scales, bias)
-        return grad_x, None, None, None, None, None, None
+        codes, codebooks, scales, bias, x = ctx.saved_tensors
+        grad_x = grad_codebooks = grad_scales = grad_bias = None
+        if ctx.needs_input_grad[0]:
+            grad_x = ctx.backward_op(grad_y, codes, codebooks, scales, bias)
+        if ctx.needs_input_grad[2] or ctx.needs_input_grad[3]:
+            from .inference_kernels import cuda_kernel
+
+            grad_codebooks, grad_scales = cuda_kernel.matmat_weight_grad(x, grad_y, codes, codebooks, scales,
+                                                                         ctx.needs_input_grad[2], ctx.needs_input_grad[3])
+        if ctx.needs_input_grad[4]:
+            grad_bias = grad_y.reshape(-1, grad_y.shape[-1]).sum(dim=0, dtype=torch.float32).to(bias.dtype)
+        return grad_x, None, grad_codebooks, grad_scales, grad_bias, None, None
+
+
+def weights_require_grad(m) -> bool:
+    """True when any of a quantized linear's trainable parameters (codebooks, scales, bias) requires a gradient."""
+    return m.codebooks.requires_grad or m.scales.requires_grad or (m.bias is not None and m.bias.requires_grad)
 
 
 def _frozen(shape, **kwargs) -> nn.Parameter:
@@ -108,7 +125,7 @@ class QuantizedLinear(nn.Module):
         if self._ops is None:
             self.prepare_matmul_op(input)
         fwd, bwd = self._ops[:2] if self.use_gemv_rule(input) else self._ops[2:]
-        if not (torch.is_grad_enabled() and input.requires_grad):
+        if not (torch.is_grad_enabled() and (input.requires_grad or weights_require_grad(self))):
             return fwd(input, self.codes, self.codebooks, self.scales, self.bias)  # inference: skip the autograd node
         return _AqlmMatmul.apply(input, self.codes, self.codebooks, self.scales, self.bias, fwd, bwd)
 

@@ -12,6 +12,7 @@ from __future__ import annotations
 
 import ctypes
 import os
+import warnings
 from types import SimpleNamespace
 from typing import Optional
 
@@ -364,6 +365,82 @@ def matmat_dequant_transposed_routed(grad_out, codes, codebooks_stacked, scales,
         return None
     _cabi.check(rc)
     return out
+
+
+def _check_deterministic_codebook_grad() -> None:
+    """torch's rule for nondeterministic CUDA ops: raise under torch.use_deterministic_algorithms(True), warn with
+    warn_only=True."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return
+    msg = ("aqlm_b200 matmat_weight_grad: the codebook gradient is summed with atomic reductions and is not "
+           "deterministic (its last bits depend on arrival order); the scale gradient is deterministic")
+    if torch.is_deterministic_algorithms_warn_only_enabled():
+        warnings.warn(msg)
+    else:
+        raise RuntimeError(msg)
+
+
+def _weight_grad_dense(flat_x, flat_g, codes, codebooks, scales, want_codebooks, want_scales):
+    """The same quantities through a materialised W, for layouts the fused kernel does not take (in_group 16, 3
+    codebooks, unaligned views): Wu = dequant (unscaled), D = G^T X in fp32, a row dot and an index_add_ over the codes."""
+    K, cb_size, _, g = codebooks.shape
+    out_f = flat_g.shape[1]
+    D = flat_g.float().t() @ flat_x.float()  # [out, in]
+    gs = gcb = None
+    if want_scales:
+        gs = (D * dequant(codes, codebooks, None).float()).sum(dim=1)
+    if want_codebooks:
+        sD = (D * scales.reshape(-1, 1).float()).reshape(-1, g)  # [out * in / g, g]
+        c = codes.reshape(out_f, -1, K).long() % cb_size           # unsigned codes [out, in / g, K]
+        gcb = torch.zeros((K, cb_size, g), dtype=torch.float32, device=D.device)
+        for k in range(K):
+            gcb[k].index_add_(0, c[:, :, k].reshape(-1), sD)
+    return gcb, gs
+
+
+def matmat_weight_grad(x, grad_y, codes, codebooks, scales, want_codebooks: bool = True, want_scales: bool = True):
+    """Gradients of a quantized linear's codebooks and scales from its input `x` [..., in] and output gradient `grad_y`
+    [..., out], in ONE fused wgmma GEMM (csrc/gemm_wgrad.cuh) that never materialises W or dW:
+      grad_codebooks[k, c, 0, i] = sum over (r, g) with code(r, g, k) = c of scales[r] * (grad_y^T x)[r, 8 g + i]
+      grad_scales[r]             = sum_j (grad_y^T x)[r, j] * Wu[r, j]     (Wu: the unscaled weight)
+    Returns (grad_codebooks, grad_scales) with the parameters' shapes and dtypes, accumulated in fp32 and rounded once;
+    either is None when not wanted.  Layouts the kernel refuses go through a dense formulation (dequant + matmul +
+    index_add_).  The codebook gradient is not deterministic (atomic fp32 sums): under
+    torch.use_deterministic_algorithms(True) requesting it raises (warns with warn_only=True)."""
+    device = _require_cuda(x, grad_y, codes, codebooks, scales)
+    _dtype_code(x)
+    if x.dtype != codebooks.dtype or grad_y.dtype != codebooks.dtype:
+        raise ValueError(f"input {x.dtype} / grad_output {grad_y.dtype} must match the codebooks' dtype {codebooks.dtype}")
+    if want_codebooks:
+        _check_deterministic_codebook_grad()
+    w = make_weight(codes, codebooks, scales.reshape(-1), None)
+    if x.shape[-1] != w.in_features or grad_y.shape[-1] != w.out_features or x.shape[:-1] != grad_y.shape[:-1]:
+        raise ValueError(f"input {tuple(x.shape)} / grad_output {tuple(grad_y.shape)} do not match a "
+                         f"{w.in_features} -> {w.out_features} linear")
+    flat_x = x.reshape(-1, w.in_features)
+    flat_g = grad_y.reshape(-1, w.out_features)
+    flat_x = flat_x if flat_x.is_contiguous() else flat_x.contiguous()
+    flat_g = flat_g if flat_g.is_contiguous() else flat_g.contiguous()
+    batch = flat_x.shape[0]
+    K, cb_size, _, g = codebooks.shape
+    gcb = torch.zeros((K, cb_size, g), dtype=torch.float32, device=device) if want_codebooks else None
+    gs = torch.zeros((w.out_features,), dtype=torch.float32, device=device) if want_scales else None
+    if batch > 0 and (want_codebooks or want_scales):
+        with _on_device(device):
+            L = _cabi.lib()
+            need = L.aqlm_b200_matmat_weight_grad_workspace_bytes(ctypes.byref(w), batch) if want_scales else 0
+            ws = _workspace(device, need) if need else None
+            rc = L.aqlm_b200_matmat_weight_grad(ctypes.byref(w), flat_x.data_ptr(), flat_g.data_ptr(), batch,
+                                                gcb.data_ptr() if gcb is not None else None,
+                                                gs.data_ptr() if gs is not None else None,
+                                                ws.data_ptr() if ws is not None else None,
+                                                ws.numel() if ws is not None else 0, _stream_ptr(device))
+        if rc == _cabi.ERR_UNSUPPORTED:
+            gcb, gs = _weight_grad_dense(flat_x, flat_g, codes, codebooks, scales, want_codebooks, want_scales)
+        else:
+            _cabi.check(rc)
+    return (None if gcb is None else gcb.reshape(codebooks.shape).to(codebooks.dtype),
+            None if gs is None else gs.reshape(scales.shape).to(scales.dtype))
 
 
 def matmat_partial(input, codes, codebooks) -> torch.Tensor:

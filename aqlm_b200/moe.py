@@ -29,7 +29,7 @@ import torch
 from torch import nn
 
 from .grouped import gemm_scheme
-from .inference import QuantizedLinear
+from .inference import QuantizedLinear, weights_require_grad
 
 
 def route(top_k_index: torch.Tensor, n_experts: int) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
@@ -129,7 +129,10 @@ class QuantizedMixtralExperts(nn.Module):
 
     # -- forward ------------------------------------------------------------------------------------------------------
     def forward(self, hidden_states: torch.Tensor, top_k_index: torch.Tensor, top_k_weights: torch.Tensor) -> torch.Tensor:
-        if self.routed and hidden_states.is_cuda:
+        # trainable codebooks / scales: the members' own autograd nodes (no routed weight-gradient kernel)
+        train_weights = torch.is_grad_enabled() and any(weights_require_grad(m) for m in self.modules()
+                                                        if isinstance(m, QuantizedLinear))
+        if self.routed and hidden_states.is_cuda and not train_weights:
             out = self._forward_routed(hidden_states, top_k_index, top_k_weights)
             if out is not None:
                 return out

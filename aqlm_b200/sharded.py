@@ -19,6 +19,7 @@ import torch
 import torch.distributed as dist
 import torch.nn as nn
 
+from .inference import weights_require_grad
 from .utils import get_int_dtype
 
 
@@ -94,6 +95,8 @@ class ShardedQuantizedLinear(nn.Module):
 
     def forward(self, input: torch.Tensor) -> torch.Tensor:
         """`input` is either the full [..., in_features] activation or this rank's [..., in_features/W] slice."""
+        if torch.is_grad_enabled() and weights_require_grad(self):
+            raise NotImplementedError("the sharded path has no weight gradient: freeze codebooks, scales and bias")
         injected = self._partial_fn is not None and not getattr(self, "_default_fns", False)
         partial_fn, epilogue_fn = self._compute_fns()
         local = self.in_end - self.in_begin

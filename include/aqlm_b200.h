@@ -174,6 +174,24 @@ int aqlm_b200_matmat_dequant_transposed_routed(const aqlm_b200_weight_t* w, cons
                                                void* grad_input, int64_t rows, void* workspace, size_t workspace_bytes,
                                                void* stream);
 
+/* ---- weight gradient: the gradients of a linear's codebooks and scales in ONE fused wgmma GEMM ----------------
+ * With D = grad_output^T . input [out, in] (fp32) and Wu the unscaled weight as the forward computes it:
+ *   grad_codebooks[k][c][i] += sum over (r, g) with code(r, g, k) = c of scales[r] * D[r, 8 g + i]
+ *   grad_scales[r]           = sum_j D[r, j] * Wu[r, j]
+ * input [batch, in] and grad_output [batch, out] in w->dtype.  grad_codebooks is fp32 [K][2^nbits][8] and the call ADDS
+ * into it (the caller zeroes it, or accumulates); grad_scales is fp32 [out] and is WRITTEN.  Either may be NULL (not
+ * wanted), not both; w->scales is required with grad_codebooks.  grad_scales needs the workspace of
+ * aqlm_b200_matmat_weight_grad_workspace_bytes (counters, left at zero, and per-tile row dots).  grad_scales is
+ * deterministic; grad_codebooks is summed in atomic arrival order (fp32, denormals flushed), so its last bits can
+ * differ from run to run.  Errors, before any device query: AQLM_B200_ERR_SHAPE for a bad descriptor, NULL input /
+ * grad_output or both outputs NULL; AQLM_B200_ERR_UNSUPPORTED for layouts the kernel does not take (in_group 16,
+ * codebook counts other than 1/2/4/8, codes other than 8/16-bit, code rows not 16-byte aligned, out_features % 8 != 0,
+ * input or grad_output not 16-byte aligned).  batch == 0: OK, no launch.  Exactly one launch otherwise. */
+size_t aqlm_b200_matmat_weight_grad_workspace_bytes(const aqlm_b200_weight_t* w, int64_t batch);
+int aqlm_b200_matmat_weight_grad(const aqlm_b200_weight_t* w, const void* input, const void* grad_output,
+                                 int64_t batch, float* grad_codebooks, float* grad_scales, void* workspace,
+                                 size_t workspace_bytes, void* stream);
+
 /* Epilogue of the sharded path: output[b,o] = (T)(partial[b,o] * scales[o] + bias[o]) after the
  * all-reduce of the fp32 partials (new work; the reference has no multi-GPU hot path, SURVEY §8e). */
 int aqlm_b200_scale_bias(const float* partial, const void* scales, const void* bias, void* output, int64_t batch,
