@@ -107,18 +107,20 @@ static int with_batch_tile(int64_t rows, F&& f) {
   return f(Int<8>{});
 }
 
-// (codebooks, code bytes) of the wgmma GEMMs: K in {1, 2, 4, 8}, 8- or 16-bit codes
+// (dtype, codebooks, code bytes) of the wgmma GEMMs: K in {1, 2, 4, 8}, 8- or 16-bit codes
 template <typename F>
 static int with_gemm_scheme(const aqlm_b200_weight_t* w, F&& f) {
-  const auto k = [&](auto CB) {
-    switch (w->num_codebooks) {
-      case 1: return f(Int<1>{}, CB);
-      case 2: return f(Int<2>{}, CB);
-      case 4: return f(Int<4>{}, CB);
-      default: return f(Int<8>{}, CB);
-    }
-  };
-  return w->nbits_per_codebook <= 8 ? k(Int<1>{}) : k(Int<2>{});
+  return with_dtype(w->dtype, [&](auto tag) {
+    const auto k = [&](auto CB) {
+      switch (w->num_codebooks) {
+        case 1: return f(tag, Int<1>{}, CB);
+        case 2: return f(tag, Int<2>{}, CB);
+        case 4: return f(tag, Int<4>{}, CB);
+        default: return f(tag, Int<8>{}, CB);
+      }
+    };
+    return w->nbits_per_codebook <= 8 ? k(Int<1>{}) : k(Int<2>{});
+  });
 }
 
 // wgmma N of a GEMM plan: 16, 32, 64 or 128
@@ -483,33 +485,42 @@ static int encode_tmap(CUtensorMap* map, const char* what, CUtensorMapDataType t
 template <typename T>
 constexpr CUtensorMapDataType kTmapType = DT<T>::is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
 
-// One launch of either GEMM.  Forward: b = x [batch][in_features], y [batch][out_features] (fp32 sums with `partial`).
-// TRANSPOSED (backward w.r.t. the input): b = grad_output [batch][out_features], y = grad_input [batch][in_features].
-// The directions differ in the code-tile map and in which side of W is the contraction; the rest is shared.
-// Segments of the out rows (GemmParams::n_seg / seg_end): one for a plain linear, up to 4 for a grouped call.
-struct GemmSegments {
-  int n_seg = 1;
-  int seg_end[4] = {0, 0, 0, 0};
+// One call of the fused dequant + wgmma GEMM.  Forward: b = x [rows][in_features], y [rows][out_features] (fp32 sums
+// with `partial`).  Transposed (backward w.r.t. the input): b = grad_output [rows][out_features], y = grad_input
+// [rows][in_features].  The directions differ in the code-tile map and in which side of W is the contraction; the rest
+// is shared.  Segments of the out rows (GemmParams::n_seg / seg_end): one for a plain linear, up to 4 for a grouped or
+// routed call.  A routed call (n_experts > 0) covers n_experts stacked experts of w's shape: the code map spans all of
+// them, and expert e takes the rows [expert_off[e], expert_off[e+1]).
+struct GemmCall {
+  const aqlm_b200_weight_t* w;
+  const void* b;
+  void* y;
+  int64_t rows;
+  bool transposed, partial;
+  int n_seg;
+  int seg_end[4];
+  const int32_t* expert_off;
+  int n_experts;
 };
 
-static GemmSegments single_segment(const aqlm_b200_weight_t* w) {
-  GemmSegments s;
-  for (int& e : s.seg_end) e = (int)w->out_features;
-  return s;
+// A call on one validated plain linear: one segment, not routed.
+static GemmCall plain_gemm_call(const aqlm_b200_weight_t* w, const void* b, void* y, int64_t rows, bool transposed,
+                                bool partial) {
+  const int out = (int)w->out_features;
+  return {w, b, y, rows, transposed, partial, 1, {out, out, out, out}, nullptr, 0};
 }
 
-// A routed call (expert_off != NULL) covers n_experts stacked experts of w's shape: the code map spans all of them.
 template <typename T, int K, int CB, bool TRANSPOSED>
-static int launch_gemm(const aqlm_b200_weight_t* w, const void* b, void* y, int64_t batch, bool partial, const GemmPlan& g,
-                       const GemmSegments& segs, void* workspace, const DeviceInfo* di, cudaStream_t st,
-                       const int32_t* expert_off = nullptr, int n_experts = 1) {
+static int launch_gemm(const GemmCall& c, const GemmPlan& g, void* workspace, const DeviceInfo* di, cudaStream_t st) {
   using Dir = std::conditional_t<TRANSPOSED, GemmTransposed<K, CB>, GemmForward<K, CB>>;
+  const aqlm_b200_weight_t* w = c.w;
   const int64_t k_size = TRANSPOSED ? w->out_features : w->in_features;
   const size_t row_bytes = (size_t)(w->in_features / 8) * K * CB;
   CUtensorMap tb, tc;
-  if (int rc = encode_tmap(&tb, TRANSPOSED ? "grad_output" : "x", kTmapType<T>, b, k_size, batch, k_size * 2, kGemmBlockK,
-                           g.n_tile, CU_TENSOR_MAP_SWIZZLE_128B))
+  if (int rc = encode_tmap(&tb, TRANSPOSED ? "grad_output" : "x", kTmapType<T>, c.b, k_size, c.rows, k_size * 2,
+                           kGemmBlockK, g.n_tile, CU_TENSOR_MAP_SWIZZLE_128B))
     return rc;
+  const int n_experts = c.n_experts > 0 ? c.n_experts : 1;  // the experts the code map spans
   const uint64_t code_rows = (uint64_t)w->out_features * (uint64_t)n_experts;
   if (int rc = TRANSPOSED ? encode_tmap(&tc, "codes, transposed", CU_TENSOR_MAP_DATA_TYPE_UINT8, w->codes, row_bytes,
                                         code_rows, row_bytes, 16 * K * CB, kGemmTCtileRows, CU_TENSOR_MAP_SWIZZLE_NONE)
@@ -518,39 +529,72 @@ static int launch_gemm(const aqlm_b200_weight_t* w, const void* b, void* y, int6
     return rc;
   GemmParams p;
   p.codebooks = w->codebooks;
-  p.scales = partial ? nullptr : w->scales;
-  p.bias = partial || TRANSPOSED ? nullptr : w->bias;
-  p.partial_f32 = partial ? 1 : 0;
-  p.y = y;
+  p.scales = c.partial ? nullptr : w->scales;
+  p.bias = c.partial || TRANSPOSED ? nullptr : w->bias;
+  p.partial_f32 = c.partial ? 1 : 0;
+  p.y = c.y;
   p.ws_counters = g.ksplit > 1 ? reinterpret_cast<unsigned int*>(workspace) : nullptr;
   p.ws_partials = g.ksplit > 1 ? reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + g.counters_bytes) : nullptr;
   p.m_size = (int)(TRANSPOSED ? w->in_features : w->out_features);
   p.k_size = (int)k_size;
-  p.batch = (int)batch;
+  p.batch = (int)c.rows;
   p.nbits = w->nbits_per_codebook;
   p.total_kblocks = g.total_kblocks;
   p.ksplit = g.ksplit;
   p.stages = g.stages;
   p.tile_m = g.tile_m;
   p.gather_mode = tun().gemm_gather_mode >= 0 ? tun().gemm_gather_mode : (w->nbits_per_codebook > 8 ? 1 : 0);
-  p.n_seg = segs.n_seg;
-  for (int i = 0; i < 4; ++i) p.seg_end[i] = segs.seg_end[i];
-  p.expert_off = expert_off;
+  p.n_seg = c.n_seg;
+  for (int i = 0; i < 4; ++i) p.seg_end[i] = c.seg_end[i];
+  p.expert_off = c.expert_off;
   p.n_experts = n_experts;
   return with_n_tile(g.n_tile, [&](auto N) {
     const dim3 grid(g.m_tiles, g.ksplit, g.n_tiles);  // routed: n_tiles is the slot count
     const size_t smem = gemm_smem_layout(g.stages, N, Dir::kCtileBytes).total;
-    if (expert_off) {
+    if (c.n_experts > 0) {
       constexpr auto kernel = TRANSPOSED ? gemm_dequant_t_routed_kernel<T, K, CB, N> : gemm_dequant_routed_kernel<T, K, CB, N>;
       return launch<kernel>(di, grid, kGemmThreads, smem, st, 0, tb, tc, p);
     }
-    if (segs.n_seg > 1) {
+    if (c.n_seg > 1) {
       constexpr auto kernel = TRANSPOSED ? gemm_dequant_t_grouped_kernel<T, K, CB, N> : gemm_dequant_grouped_kernel<T, K, CB, N>;
       return launch<kernel>(di, grid, kGemmThreads, smem, st, 0, tb, tc, p);
     }
     constexpr auto kernel = TRANSPOSED ? gemm_dequant_t_kernel<T, K, CB, N> : gemm_dequant_kernel<T, K, CB, N>;
     return launch<kernel>(di, grid, kGemmThreads, smem, st, 0, tb, tc, p);
   });
+}
+
+// What run_gemm returns when no wgmma plan covers the call: the caller falls back or fails with its own message.
+constexpr int kNoGemmPlan = -1;
+
+// Everything a GEMM call does after its argument checks: plan on the current device (split-K only with a workspace, and
+// without a split when the workspace is too small for the plan's), then one launch.
+static int run_gemm(const GemmCall& c, void* workspace, size_t workspace_bytes, void* stream) {
+  const DeviceInfo* di;
+  if (int rc = current_device(&di)) return rc;
+  const auto plan = [&](bool split) { return gemm_plan(*c.w, c.rows, c.transposed, c.n_experts, *di, tun(), split); };
+  GemmPlan g = plan(workspace != nullptr);
+  if (g.ok && g.ksplit > 1 && workspace_bytes < g.counters_bytes + g.partials_bytes) g = plan(false);
+  if (!g.ok) return kNoGemmPlan;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return with_gemm_scheme(c.w, [&](auto tag, auto K, auto CB) {
+    using T = typename decltype(tag)::type;
+    return c.transposed ? launch_gemm<T, K, CB, true>(c, g, workspace, di, st)
+                        : launch_gemm<T, K, CB, false>(c, g, workspace, di, st);
+  });
+}
+
+constexpr int kRoutedMaxExperts = 64;
+
+// Workspace of a GEMM call (n_experts > 0: routed) with split-K allowed: the plan's counters and partials when it
+// splits, else 0.  0 as well without a device, for a descriptor validate() refuses, rows <= 0 or too many experts.
+static size_t gemm_workspace_bytes(const aqlm_b200_weight_t* w, int64_t rows, bool transposed, int n_experts,
+                                   bool need_scales) {
+  if (validate(w, need_scales) != AQLM_B200_OK || rows <= 0 || n_experts > kRoutedMaxExperts) return 0;
+  const DeviceInfo* di = device_info();
+  if (!di) return 0;
+  const GemmPlan g = gemm_plan(*w, rows, transposed, n_experts, *di, tun(), true);
+  return g.ok && g.ksplit > 1 ? g.counters_bytes + g.partials_bytes : 0;
 }
 
 static aqlm_b200_weight_t make_weight(const void* codes, const void* codebooks, const void* scales, const void* bias,
@@ -571,132 +615,78 @@ static aqlm_b200_weight_t make_weight(const void* codes, const void* codebooks, 
   return w;
 }
 
-// ---- grouped wgmma GEMM (forward and transposed): host side -----------------------------------------------------
-// Everything a grouped GEMM call checks without a device, in this order: arguments and segment table (ERR_SHAPE), then
-// the layouts the wgmma kernels take (ERR_UNSUPPORTED).  There is no GEMV form of a grouped call above 8 rows, so a
-// layout the kernels do not take is an error the caller handles (by running the members one by one).
-// The segment table of a grouped or routed call (ERR_SHAPE).
-static int gemm_segment_table(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, const char* what,
-                              GemmSegments* segs) {
-  if (!seg_rows || n_seg < 1 || n_seg > 4) return fail(AQLM_B200_ERR_SHAPE, "%s GEMM takes 1..4 segments, got %d", what, n_seg);
+// ---- argument checks of the grouped, routed and weight-gradient calls ----------------------------------------------
+// The segment table of a grouped or routed call, GEMM or GEMV: 1..4 positive row counts that add up to out_features
+// (ERR_SHAPE otherwise).  seg_end[i] is the end of segment i, and out_features past the last one.
+static int segment_table(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, const char* what,
+                         int* seg_end) {
+  if (!seg_rows || n_seg < 1 || n_seg > 4) return fail(AQLM_B200_ERR_SHAPE, "%s takes 1..4 segments, got %d", what, n_seg);
   int64_t acc = 0;
   for (int i = 0; i < n_seg; ++i) {
     if (seg_rows[i] <= 0) return fail(AQLM_B200_ERR_SHAPE, "segment %d has %lld rows", i, (long long)seg_rows[i]);
     acc += seg_rows[i];
     if (acc > w->out_features) break;
-    segs->seg_end[i] = (int)acc;
+    seg_end[i] = (int)acc;
   }
   if (acc != w->out_features)
     return fail(AQLM_B200_ERR_SHAPE, "segment rows do not add up to out_features (%lld)", (long long)w->out_features);
-  for (int i = n_seg; i < 4; ++i) segs->seg_end[i] = (int)acc;
-  segs->n_seg = n_seg;
+  for (int i = n_seg; i < 4; ++i) seg_end[i] = (int)acc;
   return AQLM_B200_OK;
 }
 
-// The layouts the wgmma kernels of a grouped or routed call take (ERR_UNSUPPORTED otherwise).
+// The layouts the wgmma kernels take (ERR_UNSUPPORTED otherwise): the schemes of gemm_scheme_ok, the direction's row
+// rule, and a 16-byte aligned b, the operand loaded by TMA (the input forward, grad_output transposed).
 static int gemm_layout_checks(const aqlm_b200_weight_t* w, const void* b, bool transposed, const char* what) {
-  const int K = w->num_codebooks, nbits = w->nbits_per_codebook, cb = nbits <= 8 ? 1 : 2;
-  if (w->in_group_size != 8 || (nbits != 8 && nbits != 16) || !(K == 1 || K == 2 || K == 4 || K == 8))
+  if (!gemm_scheme_ok(*w))
     return fail(AQLM_B200_ERR_UNSUPPORTED,
-                "%s GEMM covers in_group_size 8, 8/16-bit codes and 1/2/4/8 codebooks; got %dx%d, in_group_size %d",
-                what, K, nbits, w->in_group_size);
+                "%s covers in_group_size 8, 8/16-bit codes, 1/2/4/8 codebooks and 16-byte aligned code rows; got %dx%d, "
+                "in_group_size %d", what, w->num_codebooks, w->nbits_per_codebook, w->in_group_size);
   if (!transposed && w->in_features % kGemmBlockK != 0)
-    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s GEMM needs in_features %% 64 == 0, got %lld", what,
-                (long long)w->in_features);
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s needs in_features %% 64 == 0, got %lld", what, (long long)w->in_features);
   if (transposed && w->out_features % 8 != 0)
-    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s transposed GEMM needs out_features %% 8 == 0, got %lld", what,
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s needs out_features %% 8 == 0, got %lld", what,
                 (long long)w->out_features);
-  if (((size_t)(w->in_features / 8) * K * cb) % 16 != 0 || (reinterpret_cast<uintptr_t>(w->codes) & 15) != 0)
-    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s GEMM needs 16-byte aligned code rows", what);
   if ((reinterpret_cast<uintptr_t>(b) & 15) != 0)
-    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s GEMM needs a 16-byte aligned %s", what, transposed ? "grad_output" : "input");
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s needs a 16-byte aligned %s", what, transposed ? "grad_output" : "input");
   return AQLM_B200_OK;
 }
 
-static int grouped_gemm_checks(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, const void* b,
-                               const void* y, int64_t batch, bool partial, bool transposed, GemmSegments* segs) {
-  int rc = validate(w, !partial);
+// Everything a grouped GEMM call checks without a device, in this order: arguments and segment table (ERR_SHAPE), then
+// the layouts the wgmma kernels take (ERR_UNSUPPORTED).  There is no GEMV form of a grouped call above 8 rows, so a
+// layout the kernels do not take is an error the caller handles (by running the members one by one).
+static int grouped_gemm_checks(GemmCall& c, const int64_t* seg_rows) {
+  int rc = validate(c.w, !c.partial);
   if (rc) return rc;
-  if (batch < 0) return fail(AQLM_B200_ERR_SHAPE, "negative batch");
-  if (!b || !y) return fail(AQLM_B200_ERR_SHAPE, "input/output pointer is NULL");
-  if ((rc = gemm_segment_table(w, seg_rows, n_seg, "grouped", segs))) return rc;
-  return gemm_layout_checks(w, b, transposed, "grouped");
+  if (c.rows < 0) return fail(AQLM_B200_ERR_SHAPE, "negative batch");
+  if (!c.b || !c.y) return fail(AQLM_B200_ERR_SHAPE, "input/output pointer is NULL");
+  if ((rc = segment_table(c.w, seg_rows, c.n_seg, "grouped GEMM", c.seg_end))) return rc;
+  return gemm_layout_checks(c.w, c.b, c.transposed, "grouped GEMM");
 }
 
-// One launch of the forward (y [batch][out], fp32 sums with `partial`) or the transposed (y = grad_input [batch][in])
-// GEMM over the row-concatenated weight, with the plan of the concatenated descriptor.
-template <bool TRANSPOSED>
-static int grouped_gemm(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, const void* b, void* y,
-                        int64_t batch, bool partial, void* workspace, size_t workspace_bytes, void* stream) {
-  GemmSegments segs;
-  int rc = grouped_gemm_checks(w, seg_rows, n_seg, b, y, batch, partial, TRANSPOSED, &segs);
-  if (rc || batch == 0) return rc;
-  const DeviceInfo* di;
-  if ((rc = current_device(&di))) return rc;
-  const auto plan = [&](bool split) {
-    return TRANSPOSED ? gemm_t_plan(*w, batch, *di, tun(), split) : gemm_plan(*w, batch, *di, tun(), split);
-  };
-  GemmPlan g = plan(workspace != nullptr);
-  if (g.ok && g.ksplit > 1 && workspace_bytes < g.counters_bytes + g.partials_bytes) g = plan(false);
-  if (!g.ok) return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped GEMM: no wgmma plan for this descriptor and batch");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return with_dtype(w->dtype, [&](auto tag) {
-    return with_gemm_scheme(w, [&](auto K, auto CB) {
-      return launch_gemm<typename decltype(tag)::type, K, CB, TRANSPOSED>(w, b, y, batch, partial, g, segs, workspace, di,
-                                                                          st);
-    });
-  });
-}
-
-// ---- routed wgmma GEMM (mixture-of-experts, forward and transposed): host side -----------------------------------
-constexpr int kRoutedMaxExperts = 64;
-
-// Everything a routed call checks without a device, in this order: descriptor, segment table, expert count, pointers
-// (ERR_SHAPE); then the layouts the wgmma kernels take (ERR_UNSUPPORTED), exactly as for a grouped call.
-static int routed_gemm_checks(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, int n_experts,
-                              const int32_t* expert_off, const void* b, const void* y, int64_t rows, bool transposed,
-                              GemmSegments* segs) {
+// Everything a routed call checks without a device, in this order: descriptor, segment table (seg_rows may be NULL for
+// one segment), expert count, pointers (ERR_SHAPE); then the layouts the wgmma kernels take (ERR_UNSUPPORTED), exactly
+// as for a grouped call.
+static int routed_gemm_checks(GemmCall& c, const int64_t* seg_rows) {
+  const aqlm_b200_weight_t* w = c.w;
   int rc = validate(w, true);
   if (rc) return rc;
-  if (rows < 0) return fail(AQLM_B200_ERR_SHAPE, "negative row count");
-  if (rows > 0x7fffffffll) return fail(AQLM_B200_ERR_SHAPE, "routed GEMM takes at most 2^31 - 1 rows");
+  if (c.rows < 0) return fail(AQLM_B200_ERR_SHAPE, "negative row count");
+  if (c.rows > 0x7fffffffll) return fail(AQLM_B200_ERR_SHAPE, "routed GEMM takes at most 2^31 - 1 rows");
   const int64_t one[1] = {w->out_features};
-  if ((rc = gemm_segment_table(w, (seg_rows || n_seg != 1) ? seg_rows : one, n_seg, "routed", segs))) return rc;
-  if (n_experts < 1 || n_experts > kRoutedMaxExperts)
-    return fail(AQLM_B200_ERR_SHAPE, "routed GEMM takes 1..%d experts, got %d", kRoutedMaxExperts, n_experts);
-  if (w->out_features * n_experts > 0x7fffffffll)  // the stacked out rows are a TMA coordinate
-    return fail(AQLM_B200_ERR_SHAPE, "routed GEMM: %d experts x %lld out rows exceed 2^31 - 1", n_experts,
+  if ((rc = segment_table(w, (seg_rows || c.n_seg != 1) ? seg_rows : one, c.n_seg, "routed GEMM", c.seg_end))) return rc;
+  if (c.n_experts < 1 || c.n_experts > kRoutedMaxExperts)
+    return fail(AQLM_B200_ERR_SHAPE, "routed GEMM takes 1..%d experts, got %d", kRoutedMaxExperts, c.n_experts);
+  if (w->out_features * c.n_experts > 0x7fffffffll)  // the stacked out rows are a TMA coordinate
+    return fail(AQLM_B200_ERR_SHAPE, "routed GEMM: %d experts x %lld out rows exceed 2^31 - 1", c.n_experts,
                 (long long)w->out_features);
-  if (!expert_off) return fail(AQLM_B200_ERR_SHAPE, "expert offsets pointer is NULL");
-  if (!b || !y) return fail(AQLM_B200_ERR_SHAPE, "input/output pointer is NULL");
-  return gemm_layout_checks(w, b, transposed, "routed");
-}
-
-template <bool TRANSPOSED>
-static int routed_gemm(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, int n_experts,
-                       const int32_t* expert_off, const void* b, void* y, int64_t rows, void* workspace,
-                       size_t workspace_bytes, void* stream) {
-  GemmSegments segs;
-  int rc = routed_gemm_checks(w, seg_rows, n_seg, n_experts, expert_off, b, y, rows, TRANSPOSED, &segs);
-  if (rc || rows == 0) return rc;
-  const DeviceInfo* di;
-  if ((rc = current_device(&di))) return rc;
-  const auto plan = [&](bool split) { return gemm_routed_plan(*w, rows, n_experts, *di, tun(), split, TRANSPOSED); };
-  GemmPlan g = plan(workspace != nullptr);
-  if (g.ok && g.ksplit > 1 && workspace_bytes < g.counters_bytes + g.partials_bytes) g = plan(false);
-  if (!g.ok) return fail(AQLM_B200_ERR_UNSUPPORTED, "routed GEMM: no wgmma plan for this descriptor and row count");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return with_dtype(w->dtype, [&](auto tag) {
-    return with_gemm_scheme(w, [&](auto K, auto CB) {
-      return launch_gemm<typename decltype(tag)::type, K, CB, TRANSPOSED>(w, b, y, rows, false, g, segs, workspace, di,
-                                                                          st, expert_off, n_experts);
-    });
-  });
+  if (!c.expert_off) return fail(AQLM_B200_ERR_SHAPE, "expert offsets pointer is NULL");
+  if (!c.b || !c.y) return fail(AQLM_B200_ERR_SHAPE, "input/output pointer is NULL");
+  return gemm_layout_checks(w, c.b, c.transposed, "routed GEMM");
 }
 
 // ---- fused weight-gradient GEMM: host side ------------------------------------------------------------------------
 // Everything a weight-gradient call checks without a device: descriptor, pointers (ERR_SHAPE), then the layouts the
-// kernel takes (ERR_UNSUPPORTED).
+// kernel takes (ERR_UNSUPPORTED): those of the transposed GEMM, whose grad_output operand it shares, and an aligned input.
 static int weight_grad_checks(const aqlm_b200_weight_t* w, const void* input, const void* grad_output, int64_t batch,
                               const float* grad_codebooks, const float* grad_scales) {
   int rc = validate(w, grad_codebooks != nullptr);
@@ -705,17 +695,9 @@ static int weight_grad_checks(const aqlm_b200_weight_t* w, const void* input, co
   if (!input || !grad_output) return fail(AQLM_B200_ERR_SHAPE, "weight gradient: input/grad_output pointer is NULL");
   if (!grad_codebooks && !grad_scales)
     return fail(AQLM_B200_ERR_SHAPE, "weight gradient: neither grad_codebooks nor grad_scales requested");
-  const int K = w->num_codebooks, nbits = w->nbits_per_codebook, cb = nbits <= 8 ? 1 : 2;
-  if (w->in_group_size != 8 || (nbits != 8 && nbits != 16) || !(K == 1 || K == 2 || K == 4 || K == 8))
-    return fail(AQLM_B200_ERR_UNSUPPORTED,
-                "weight gradient covers in_group_size 8, 8/16-bit codes and 1/2/4/8 codebooks; got %dx%d, in_group_size %d",
-                K, nbits, w->in_group_size);
-  if (w->out_features % 8 != 0)
-    return fail(AQLM_B200_ERR_UNSUPPORTED, "weight gradient needs out_features %% 8 == 0, got %lld", (long long)w->out_features);
-  if (((size_t)(w->in_features / 8) * K * cb) % 16 != 0 || (reinterpret_cast<uintptr_t>(w->codes) & 15) != 0)
-    return fail(AQLM_B200_ERR_UNSUPPORTED, "weight gradient needs 16-byte aligned code rows");
-  if ((reinterpret_cast<uintptr_t>(input) & 15) != 0 || (reinterpret_cast<uintptr_t>(grad_output) & 15) != 0)
-    return fail(AQLM_B200_ERR_UNSUPPORTED, "weight gradient needs a 16-byte aligned input and grad_output");
+  if ((rc = gemm_layout_checks(w, grad_output, true, "weight gradient"))) return rc;
+  if ((reinterpret_cast<uintptr_t>(input) & 15) != 0)
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "weight gradient needs a 16-byte aligned input");
   return AQLM_B200_OK;
 }
 
@@ -840,21 +822,14 @@ int aqlm_b200_matmat_grouped(const aqlm_b200_weight_t* w, const int64_t* seg_row
     return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped launch is implemented for the 1x16 (in_group 8) scheme only");
   if (batch < 1 || batch > 8) return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped launch takes 1..8 batch rows");
   if (!input || !output) return fail(AQLM_B200_ERR_SHAPE, "input/output pointer is NULL");
-  int64_t total = 0;
-  for (int i = 0; i < n_seg; ++i) total += seg_rows[i];
-  if (total != w->out_features) return fail(AQLM_B200_ERR_SHAPE, "segment rows do not add up to out_features");
+  GemvParams p = gemv_params(w, input, output, batch, partial);
+  if ((rc = segment_table(w, seg_rows, n_seg, "grouped launch", p.seg_end))) return rc;
+  p.n_seg = n_seg;
   const size_t row_bytes = (size_t)(w->in_features / 8) * 2;
   if (row_bytes % 16 != 0 || (reinterpret_cast<uintptr_t>(w->codes) & 15) || (reinterpret_cast<uintptr_t>(input) & 15))
     return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped launch needs 16-byte aligned code rows and input");
   const DeviceInfo* di;
   if ((rc = current_device(&di))) return rc;
-  GemvParams p = gemv_params(w, input, output, batch, partial);
-  p.n_seg = n_seg;
-  int64_t acc = 0;
-  for (int i = 0; i < 4; ++i) {
-    if (i < n_seg) acc += seg_rows[i];
-    p.seg_end[i] = (int)acc;
-  }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   return with_batch_tile(batch, [&](auto BT) {
     if (vec_smem_bytes(p, 1, 2, 8, BT, false, di->sm_count) > (size_t)di->max_smem_optin - 1024)
@@ -868,12 +843,7 @@ int aqlm_b200_matmat(const aqlm_b200_weight_t* w, const void* input, void* outpu
 }
 
 size_t aqlm_b200_matmat_dequant_workspace_bytes(const aqlm_b200_weight_t* w, int64_t batch) {
-  if (validate(w, false) != AQLM_B200_OK || batch <= 0) return 0;  // the plan never reads scales
-  const DeviceInfo* di = device_info();
-  if (!di) return 0;
-  const GemmPlan g = gemm_plan(*w, batch, *di, tun(), true);
-  if (!g.ok || g.ksplit <= 1) return 0;
-  return g.counters_bytes + g.partials_bytes;
+  return gemm_workspace_bytes(w, batch, false, 0, false);  // the plan never reads scales
 }
 
 int aqlm_b200_matmat_dequant_ex(const aqlm_b200_weight_t* w, const void* input, void* output, int64_t batch,
@@ -884,22 +854,13 @@ int aqlm_b200_matmat_dequant_ex(const aqlm_b200_weight_t* w, const void* input, 
   if (batch < 0) return fail(AQLM_B200_ERR_SHAPE, "negative batch");
   if (batch == 0) return AQLM_B200_OK;
   if (!input || !output) return fail(AQLM_B200_ERR_SHAPE, "input/output pointer is NULL");
-  const DeviceInfo* di;
-  if ((rc = current_device(&di))) return rc;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  GemmPlan g = gemm_plan(*w, batch, *di, tun(), workspace != nullptr);
-  if (g.ok && g.ksplit > 1 && workspace_bytes < g.counters_bytes + g.partials_bytes) g = gemm_plan(*w, batch, *di, tun(), false);
-  if (!g.ok || (reinterpret_cast<uintptr_t>(input) & 15) != 0) {
-    // shapes the tensor-core kernel does not cover (in_group 16, in_features % 64 != 0, odd KxN):
-    // batch passes of 8 rows through the fused gather+dequant+dot kernel
-    return aqlm_b200_matmat_ex(w, input, output, batch, flags, stream);
+  if ((reinterpret_cast<uintptr_t>(input) & 15) == 0) {
+    rc = run_gemm(plain_gemm_call(w, input, output, batch, false, partial), workspace, workspace_bytes, stream);
+    if (rc != kNoGemmPlan) return rc;
   }
-  return with_dtype(w->dtype, [&](auto tag) {
-    return with_gemm_scheme(w, [&](auto K, auto CB) {
-      return launch_gemm<typename decltype(tag)::type, K, CB, false>(w, input, output, batch, partial, g, single_segment(w),
-                                                             workspace, di, st);
-    });
-  });
+  // shapes the tensor-core kernel does not cover (in_group 16, in_features % 64 != 0, odd KxN) and unaligned inputs:
+  // batch passes of 8 rows through the fused gather+dequant+dot kernel
+  return aqlm_b200_matmat_ex(w, input, output, batch, flags, stream);
 }
 
 int aqlm_b200_matmat_dequant_ws(const aqlm_b200_weight_t* w, const void* input, void* output, int64_t batch,
@@ -926,12 +887,7 @@ int aqlm_b200_dequant(const aqlm_b200_weight_t* w, void* weight_out, int apply_s
 }
 
 size_t aqlm_b200_matmat_dequant_transposed_workspace_bytes(const aqlm_b200_weight_t* w, int64_t batch) {
-  if (validate(w, true) != AQLM_B200_OK || batch <= 0) return 0;
-  const DeviceInfo* di = device_info();
-  if (!di) return 0;
-  const GemmPlan g = gemm_t_plan(*w, batch, *di, tun(), true);
-  if (!g.ok || g.ksplit <= 1) return 0;
-  return g.counters_bytes + g.partials_bytes;
+  return gemm_workspace_bytes(w, batch, true, 0, true);
 }
 
 int aqlm_b200_matmat_dequant_transposed(const aqlm_b200_weight_t* w, const void* grad_output, void* grad_input,
@@ -943,59 +899,57 @@ int aqlm_b200_matmat_dequant_transposed(const aqlm_b200_weight_t* w, const void*
   if (!grad_output || !grad_input) return fail(AQLM_B200_ERR_SHAPE, "grad_output/grad_input pointer is NULL");
   if ((reinterpret_cast<uintptr_t>(grad_output) & 15) != 0)
     return fail(AQLM_B200_ERR_SHAPE, "grad_output must be 16-byte aligned");
-  const DeviceInfo* di;
-  if ((rc = current_device(&di))) return rc;
-  GemmPlan g = gemm_t_plan(*w, batch, *di, tun(), workspace != nullptr);
-  if (g.ok && g.ksplit > 1 && workspace_bytes < g.counters_bytes + g.partials_bytes) g = gemm_t_plan(*w, batch, *di, tun(), false);
-  if (!g.ok)
-    return fail(AQLM_B200_ERR_UNSUPPORTED,
-                "matmat_dequant_transposed: the fused kernel covers in_group_size 8, 8/16-bit codes, 1/2/4/8 codebooks, "
-                "16-byte aligned code rows and out_features %% 8 == 0");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return with_dtype(w->dtype, [&](auto tag) {
-    return with_gemm_scheme(w, [&](auto K, auto CB) {
-      return launch_gemm<typename decltype(tag)::type, K, CB, true>(w, grad_output, grad_input, batch, false, g, single_segment(w),
-                                                            workspace, di, st);
-    });
-  });
+  rc = run_gemm(plain_gemm_call(w, grad_output, grad_input, batch, true, false), workspace, workspace_bytes, stream);
+  if (rc != kNoGemmPlan) return rc;
+  return fail(AQLM_B200_ERR_UNSUPPORTED,
+              "matmat_dequant_transposed: the fused kernel covers in_group_size 8, 8/16-bit codes, 1/2/4/8 codebooks, "
+              "16-byte aligned code rows and out_features %% 8 == 0");
 }
 
 int aqlm_b200_matmat_dequant_grouped(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, const void* input,
                                      void* output, int64_t batch, uint32_t flags, void* workspace, size_t workspace_bytes,
                                      void* stream) {
-  return grouped_gemm<false>(w, seg_rows, n_seg, input, output, batch, (flags & AQLM_B200_FLAG_PARTIAL_F32) != 0,
-                             workspace, workspace_bytes, stream);
+  GemmCall c = {w, input, output, batch, false, (flags & AQLM_B200_FLAG_PARTIAL_F32) != 0, n_seg, {}, nullptr, 0};
+  int rc = grouped_gemm_checks(c, seg_rows);
+  if (rc || batch == 0) return rc;
+  if ((rc = run_gemm(c, workspace, workspace_bytes, stream)) != kNoGemmPlan) return rc;
+  return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped GEMM: no wgmma plan for this descriptor and batch");
 }
 
 int aqlm_b200_matmat_dequant_transposed_grouped(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg,
                                                 const void* grad_output, void* grad_input, int64_t batch, void* workspace,
                                                 size_t workspace_bytes, void* stream) {
-  return grouped_gemm<true>(w, seg_rows, n_seg, grad_output, grad_input, batch, false, workspace, workspace_bytes, stream);
+  GemmCall c = {w, grad_output, grad_input, batch, true, false, n_seg, {}, nullptr, 0};
+  int rc = grouped_gemm_checks(c, seg_rows);
+  if (rc || batch == 0) return rc;
+  if ((rc = run_gemm(c, workspace, workspace_bytes, stream)) != kNoGemmPlan) return rc;
+  return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped GEMM: no wgmma plan for this descriptor and batch");
 }
 
 size_t aqlm_b200_matmat_dequant_routed_workspace_bytes(const aqlm_b200_weight_t* w, int n_experts, int64_t rows,
                                                        int transposed) {
-  if (validate(w, false) != AQLM_B200_OK || rows <= 0 || n_experts < 1 || n_experts > kRoutedMaxExperts) return 0;
-  const DeviceInfo* di = device_info();
-  if (!di) return 0;
-  const GemmPlan g = gemm_routed_plan(*w, rows, n_experts, *di, tun(), true, transposed != 0);
-  if (!g.ok || g.ksplit <= 1) return 0;
-  return g.counters_bytes + g.partials_bytes;
+  return n_experts < 1 ? 0 : gemm_workspace_bytes(w, rows, transposed != 0, n_experts, false);
 }
 
 int aqlm_b200_matmat_dequant_routed(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, int n_experts,
                                     const int32_t* expert_offsets, const void* input, void* output, int64_t rows,
                                     void* workspace, size_t workspace_bytes, void* stream) {
-  return routed_gemm<false>(w, seg_rows, n_seg, n_experts, expert_offsets, input, output, rows, workspace,
-                            workspace_bytes, stream);
+  GemmCall c = {w, input, output, rows, false, false, n_seg, {}, expert_offsets, n_experts};
+  int rc = routed_gemm_checks(c, seg_rows);
+  if (rc || rows == 0) return rc;
+  if ((rc = run_gemm(c, workspace, workspace_bytes, stream)) != kNoGemmPlan) return rc;
+  return fail(AQLM_B200_ERR_UNSUPPORTED, "routed GEMM: no wgmma plan for this descriptor and row count");
 }
 
 int aqlm_b200_matmat_dequant_transposed_routed(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg,
                                                int n_experts, const int32_t* expert_offsets, const void* grad_output,
                                                void* grad_input, int64_t rows, void* workspace, size_t workspace_bytes,
                                                void* stream) {
-  return routed_gemm<true>(w, seg_rows, n_seg, n_experts, expert_offsets, grad_output, grad_input, rows, workspace,
-                           workspace_bytes, stream);
+  GemmCall c = {w, grad_output, grad_input, rows, true, false, n_seg, {}, expert_offsets, n_experts};
+  int rc = routed_gemm_checks(c, seg_rows);
+  if (rc || rows == 0) return rc;
+  if ((rc = run_gemm(c, workspace, workspace_bytes, stream)) != kNoGemmPlan) return rc;
+  return fail(AQLM_B200_ERR_UNSUPPORTED, "routed GEMM: no wgmma plan for this descriptor and row count");
 }
 
 size_t aqlm_b200_matmat_weight_grad_workspace_bytes(const aqlm_b200_weight_t* w, int64_t batch) {
@@ -1019,11 +973,9 @@ int aqlm_b200_matmat_weight_grad(const aqlm_b200_weight_t* w, const void* input,
     return fail(AQLM_B200_ERR_SHAPE, "weight gradient: grad_scales needs a workspace of %zu bytes, got %zu",
                 g.counters_bytes + g.dots_bytes, workspace ? workspace_bytes : (size_t)0);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return with_dtype(w->dtype, [&](auto tag) {
-    return with_gemm_scheme(w, [&](auto K, auto CB) {
-      return launch_weight_grad<typename decltype(tag)::type, K, CB>(w, input, grad_output, batch, grad_codebooks,
-                                                                     grad_scales, workspace, g, di, st);
-    });
+  return with_gemm_scheme(w, [&](auto tag, auto K, auto CB) {
+    return launch_weight_grad<typename decltype(tag)::type, K, CB>(w, input, grad_output, batch, grad_codebooks,
+                                                                   grad_scales, workspace, g, di, st);
   });
 }
 
@@ -1167,16 +1119,12 @@ int aqlm_b200_matmat_allreduce(aqlm_b200_comm* c, const aqlm_b200_weight_t* w, c
   const size_t row_bytes = (size_t)(w->in_features / 8) * 2;
   if (row_bytes % 16 != 0 || (reinterpret_cast<uintptr_t>(w->codes) & 15) || (reinterpret_cast<uintptr_t>(input) & 15))
     return fail(AQLM_B200_ERR_UNSUPPORTED, "fused exchange needs 16-byte aligned code rows and input");
+  GemvParams p = gemv_params(w, input, output, batch, false);
+  const int64_t one[1] = {w->out_features};  // one segment: seg_rows is not read
+  if ((rc = segment_table(w, n_seg > 1 ? seg_rows : one, n_seg, "fused exchange", p.seg_end))) return rc;
+  p.n_seg = n_seg;
   const DeviceInfo* di;
   if ((rc = current_device(&di))) return rc;
-  GemvParams p = gemv_params(w, input, output, batch, false);
-  p.n_seg = n_seg;
-  int64_t acc = 0;
-  for (int i = 0; i < 4; ++i) {
-    if (i < n_seg) acc += (n_seg > 1 ? seg_rows[i] : w->out_features);
-    p.seg_end[i] = (int)acc;
-  }
-  if (acc != w->out_features) return fail(AQLM_B200_ERR_SHAPE, "segment rows do not add up to out_features");
   GemvPeer pc;
   for (int r = 0; r < 16; ++r) pc.peer_base[r] = r < c->world ? c->peer_base[r] : nullptr;
   pc.step = c->local_state;

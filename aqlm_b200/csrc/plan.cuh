@@ -139,14 +139,14 @@ inline double gemm_kblock_clk(int rows, int K, int nbits, int n_tile, double sme
   return (t > t_smem ? t : t_smem) + 60.0;
 }
 
-// Checks both GEMMs share: in_group 8, 8- or 16-bit codes, 1/2/4/8 codebooks, 16-byte aligned code rows.
-// TMA needs a 16-byte multiple as the global row stride of the code matrix (1x8: in_features % 128 == 0).
-inline bool gemm_scheme_ok(const aqlm_b200_weight_t& w, const Tunables& t) {
+// The schemes the wgmma GEMMs take (forward, transposed, grouped, routed, weight gradient): in_group 8, 8- or 16-bit
+// codes, 1/2/4/8 codebooks, 16-byte aligned code rows.  TMA needs a 16-byte multiple as the global row stride of the
+// code matrix (1x8: in_features % 128 == 0).
+inline bool gemm_scheme_ok(const aqlm_b200_weight_t& w) {
   const int K = w.num_codebooks, nbits = w.nbits_per_codebook, cb = nbits <= 8 ? 1 : 2;
   if (w.in_group_size != 8 || (nbits != 8 && nbits != 16) || !(K == 1 || K == 2 || K == 4 || K == 8)) return false;
   if ((reinterpret_cast<uintptr_t>(w.codes) & 15) != 0) return false;
-  if (((size_t)(w.in_features / 8) * K * cb) % 16 != 0) return false;
-  return !t.disable_wgmma;
+  return ((size_t)(w.in_features / 8) * K * cb) % 16 == 0;
 }
 
 // Pipeline depth: at most 3 stages (shared memory taken here is L1 taken from the codebook gathers, and outstanding
@@ -203,84 +203,40 @@ inline void gemm_finish(GemmPlan& g, int ks, bool allow_split, const Tunables& t
   g.ok = true;
 }
 
-// Forward: y[batch][out] = x[batch][in] W^T.  Searches the tile height (128 down to 64 in steps of 1, then to 32 in
-// steps of 8) together with the split count; AQLM_B200_GEMM_TILE_M in [8, 128] forces the height.
-inline GemmPlan gemm_plan(const aqlm_b200_weight_t& w, int64_t batch, const DeviceInfo& di, const Tunables& t,
-                          bool allow_split) {
+// One call of the fused dequant + wgmma GEMM over `rows` rows of activations:
+//   forward:    y[rows][out] = x[rows][in] W^T.  The tile height is searched (128 down to 64 in steps of 1, then to 32 in
+//               steps of 8) together with the split count; AQLM_B200_GEMM_TILE_M in [8, 128] forces it.
+//   transposed: grad_in[rows][in] = grad_out[rows][out] W (the backward w.r.t. the input), tiles of kGemmBlockM input
+//               rows.  A plain transposed call of more than kGemmMaxTiles tiles is not covered.
+// n_experts > 0: a routed (mixture-of-experts) call over n_experts experts of descriptor w's shape.  The routing is on
+// the device, so the plan assumes it balanced: N is the MMA width for ceil(rows / m) rows per expert (m = min(E, rows)
+// experts non-empty), and the tile height and split count are searched over m_tiles x the slots balanced routing keeps
+// busy.  The grid has routed_slot_count() slots, enough for any routing; the slots are the plan's n_tiles (workspace
+// [m_tiles][slots][ksplit][N][128]).  More slots than a grid dimension holds: no plan.  More than kGemmMaxTiles tiles
+// (m_tiles x slots), forward or transposed: no split.
+inline GemmPlan gemm_plan(const aqlm_b200_weight_t& w, int64_t rows, bool transposed, int n_experts, const DeviceInfo& di,
+                          const Tunables& t, bool allow_split) {
   GemmPlan g;
   const int K = w.num_codebooks, nbits = w.nbits_per_codebook;
   const int cb = nbits <= 8 ? 1 : 2;
-  if (!gemm_scheme_ok(w, t) || 8 * K * cb > kCodeTileBytes || w.in_features % kGemmBlockK != 0) return g;
-  g.total_kblocks = (int)(w.in_features / kGemmBlockK);
-  gemm_n_tiles(batch, &g.n_tile, &g.n_tiles);
-  g.stages = gemm_stages([&](int s) { return gemm_smem_layout(s, g.n_tile, kGemmBlockM * kCodeTileBytes).total; },
-                         (size_t)di.max_smem_optin, t.gemm_stages, 4);
-  if (!g.stages) return g;
-  int best_tm = kGemmBlockM, best_ks = 1;
-  double best = 1e30;
-  const int max_ks = allow_split ? gemm_max_ksplit(g.total_kblocks) : 1;
-  for (int tm = kGemmBlockM; tm >= 32; tm -= (tm > 64 ? 1 : 8)) {
-    const long long tiles = ((w.out_features + tm - 1) / tm) * (long long)g.n_tiles;
-    if (tiles > kGemmMaxTiles) continue;
-    gemm_split_search(tm, tiles, K, nbits, g.n_tile, g.total_kblocks, max_ks, di.sm_count, &best, &best_tm, &best_ks);
-  }
-  g.tile_m = best_tm;
-  if (t.gemm_tile_m >= 8 && t.gemm_tile_m <= kGemmBlockM) g.tile_m = t.gemm_tile_m;
-  g.m_tiles = (int)((w.out_features + g.tile_m - 1) / g.tile_m);
-  gemm_finish(g, best_ks, allow_split, t);  // more than kGemmMaxTiles tiles: no split
-  return g;
-}
-
-// Transposed (backward w.r.t. the input): grad_in[batch][in] = grad_out[batch][out] W.  Tiles of kGemmBlockM input
-// rows; more than kGemmMaxTiles tiles is not covered.
-inline GemmPlan gemm_t_plan(const aqlm_b200_weight_t& w, int64_t batch, const DeviceInfo& di, const Tunables& t,
-                            bool allow_split) {
-  GemmPlan g;
-  const int K = w.num_codebooks, nbits = w.nbits_per_codebook;
-  const int cb = nbits <= 8 ? 1 : 2;
-  if (!gemm_scheme_ok(w, t) || 16 * K * cb > 256) return g;
-  if (w.out_features % 8 != 0) return g;  // TMA row stride of grad_out
-  g.total_kblocks = (int)((w.out_features + kGemmBlockK - 1) / kGemmBlockK);
-  g.m_tiles = (int)((w.in_features + kGemmBlockM - 1) / kGemmBlockM);
-  gemm_n_tiles(batch, &g.n_tile, &g.n_tiles);
-  const int ctile_bytes = kGemmTCtileRows * 16 * K * cb;
-  // forced stages: 2..3, i.e. never more than the unforced choice
-  g.stages = gemm_stages([&](int s) { return gemm_smem_layout(s, g.n_tile, ctile_bytes).total; },
-                         (size_t)di.max_smem_optin, t.gemm_stages, 3);
-  if (!g.stages) return g;
-  if ((size_t)g.m_tiles * g.n_tiles > (size_t)kGemmMaxTiles) return g;
-  int best_tm = kGemmBlockM, best_ks = 1;
-  double best = 1e30;
-  if (allow_split)
-    gemm_split_search(kGemmBlockM, (long long)g.m_tiles * g.n_tiles, K, nbits, g.n_tile, g.total_kblocks,
-                      gemm_max_ksplit(g.total_kblocks), di.sm_count, &best, &best_tm, &best_ks);
-  gemm_finish(g, best_ks, allow_split, t);
-  return g;
-}
-
-// Routed (mixture-of-experts) GEMM over n_experts experts of descriptor w's shape, forward or transposed, `rows` input
-// rows in all.  The routing is on the device, so the plan assumes it balanced: N is the MMA width for ceil(rows / m)
-// rows per expert (m = min(E, rows) experts non-empty), and the tile height and split count are searched over m_tiles x
-// the slots balanced routing keeps busy.  The grid has routed_slot_count() slots, enough for any routing; the slots
-// are the plan's n_tiles (workspace [m_tiles][slots][ksplit][N][128]).  More than kGemmMaxTiles tiles: no split; more
-// slots than a grid dimension holds: no plan.
-inline GemmPlan gemm_routed_plan(const aqlm_b200_weight_t& w, int64_t rows, int n_experts, const DeviceInfo& di,
-                                 const Tunables& t, bool allow_split, bool transposed) {
-  GemmPlan g;
-  const int K = w.num_codebooks, nbits = w.nbits_per_codebook;
-  const int cb = nbits <= 8 ? 1 : 2;
-  if (rows < 1 || n_experts < 1 || !gemm_scheme_ok(w, t)) return g;
-  if (transposed ? (16 * K * cb > 256 || w.out_features % 8 != 0)
+  const bool routed = n_experts > 0;
+  if (t.disable_wgmma || !gemm_scheme_ok(w) || (routed && rows < 1)) return g;
+  if (transposed ? (16 * K * cb > 256 || w.out_features % 8 != 0)  // TMA row stride of grad_out
                  : (8 * K * cb > kCodeTileBytes || w.in_features % kGemmBlockK != 0))
     return g;
-  const int64_t m = rows < n_experts ? rows : n_experts;
-  int per_expert_tiles = 0;
-  gemm_n_tiles((rows + m - 1) / m, &g.n_tile, &per_expert_tiles);
-  const long long slots = routed_slot_count(rows, n_experts, g.n_tile);
-  if (slots > 65535) return g;
-  g.n_tiles = (int)slots;
-  const long long active = m * (long long)per_expert_tiles;
+  int64_t m = 1;  // experts non-empty under balanced routing
+  if (routed) m = rows < n_experts ? rows : n_experts;
+  int col_tiles = 0;  // tiles of N rows: of the batch, or of one balanced expert share
+  gemm_n_tiles((rows + m - 1) / m, &g.n_tile, &col_tiles);
+  const long long active = m * (long long)col_tiles;
+  g.n_tiles = col_tiles;
+  if (routed) {
+    const long long slots = routed_slot_count(rows, n_experts, g.n_tile);
+    if (slots > 65535) return g;
+    g.n_tiles = (int)slots;
+  }
   const int ctile_bytes = transposed ? kGemmTCtileRows * 16 * K * cb : kGemmBlockM * kCodeTileBytes;
+  // forced stages of the transposed kernel: 2..3, i.e. never more than the unforced choice
   g.stages = gemm_stages([&](int s) { return gemm_smem_layout(s, g.n_tile, ctile_bytes).total; },
                          (size_t)di.max_smem_optin, t.gemm_stages, transposed ? 3 : 4);
   if (!g.stages) return g;
@@ -289,8 +245,10 @@ inline GemmPlan gemm_routed_plan(const aqlm_b200_weight_t& w, int64_t rows, int 
   int best_tm = kGemmBlockM, best_ks = 1;
   double best = 1e30;
   if (transposed) {
-    gemm_split_search(kGemmBlockM, ((w.in_features + kGemmBlockM - 1) / kGemmBlockM) * active, K, nbits, g.n_tile,
-                      g.total_kblocks, max_ks, di.sm_count, &best, &best_tm, &best_ks);
+    const long long tiles = ((w.in_features + kGemmBlockM - 1) / kGemmBlockM) * active;
+    if (!routed && tiles > kGemmMaxTiles) return g;
+    gemm_split_search(kGemmBlockM, tiles, K, nbits, g.n_tile, g.total_kblocks, max_ks, di.sm_count, &best, &best_tm,
+                      &best_ks);
   } else {
     for (int tm = kGemmBlockM; tm >= 32; tm -= (tm > 64 ? 1 : 8)) {
       const long long tiles = ((w.out_features + tm - 1) / tm) * active;
@@ -300,9 +258,8 @@ inline GemmPlan gemm_routed_plan(const aqlm_b200_weight_t& w, int64_t rows, int 
     g.tile_m = best_tm;
     if (t.gemm_tile_m >= 8 && t.gemm_tile_m <= kGemmBlockM) g.tile_m = t.gemm_tile_m;
   }
-  const int64_t m_size = transposed ? w.in_features : w.out_features;
-  g.m_tiles = (int)((m_size + g.tile_m - 1) / g.tile_m);
-  gemm_finish(g, best_ks, allow_split, t);  // more than kGemmMaxTiles tiles (m_tiles x slots): no split
+  g.m_tiles = (int)(((transposed ? w.in_features : w.out_features) + g.tile_m - 1) / g.tile_m);
+  gemm_finish(g, best_ks, allow_split, t);
   return g;
 }
 
@@ -319,7 +276,7 @@ struct WgradPlan {
 // padding, and for 8-bit codes the CTA's K x 256 x 8 fp32 codebook gradient) reuses the pipeline's.
 inline WgradPlan gemm_wgrad_plan(const aqlm_b200_weight_t& w, int64_t batch, const DeviceInfo& di, const Tunables& t) {
   WgradPlan g;
-  if (batch < 1 || !gemm_scheme_ok(w, t) || w.out_features % 8 != 0) return g;
+  if (batch < 1 || t.disable_wgmma || !gemm_scheme_ok(w) || w.out_features % 8 != 0) return g;
   const int64_t out_tiles = (w.out_features + kWgradTile - 1) / kWgradTile;
   const int64_t in_tiles = (w.in_features + kWgradTile - 1) / kWgradTile;
   if (out_tiles > kGemmMaxTiles || in_tiles > 65535) return g;  // one ticket word per out tile; grid.y

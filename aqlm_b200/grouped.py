@@ -45,7 +45,9 @@ def _fuse_storage(members) -> dict:
 
 
 def gemm_scheme(m) -> bool:
-    """The schemes the grouped wgmma GEMM takes: in_group 8, 8- or 16-bit codes, 1/2/4/8 codebooks."""
+    """The schemes the wgmma GEMMs take: in_group 8, 8- or 16-bit codes, 1/2/4/8 codebooks.  Mirrors `gemm_scheme_ok`
+    in csrc/plan.cuh, so that a module can choose its path before it calls; the code-row alignment that rule adds is
+    left to the call, which refuses it with ERR_UNSUPPORTED."""
     return m.in_group_size == 8 and m.out_group_size == 1 and m.nbits_per_codebook in (8, 16) and \
         m.num_codebooks in (1, 2, 4, 8)
 

@@ -136,18 +136,45 @@ def _workspace(device: torch.device, nbytes: int) -> torch.Tensor:
     return _grow(_WORKSPACES, (device.index, _stream_ptr(device)), device, nbytes)
 
 
-def _prepare(input, codes, codebooks, scales, bias):
-    device = _require_cuda(input, codes, codebooks, scales, bias)
-    _dtype_code(input)
-    if input.dtype != codebooks.dtype:
-        raise ValueError(f"input dtype {input.dtype} != codebooks dtype {codebooks.dtype}")
-    w = make_weight(codes, codebooks, scales.reshape(-1) if scales is not None else None, bias)
-    if input.shape[-1] != w.in_features:
-        raise ValueError(f"input has {input.shape[-1]} features, weight expects {w.in_features}")
-    flat_input = input.reshape(-1, input.shape[-1])
-    if not flat_input.is_contiguous():
-        flat_input = flat_input.contiguous()
-    return device, w, flat_input
+def _operands(a, codes, codebooks, scales, bias, transposed: bool = False, extra=(), w=None):
+    """Checks and describes the operands of one call: `a` is the input [..., in], or grad_output [..., out] when
+    `transposed`; `extra` are further tensors that must be on its device; `w` is the descriptor when the caller has
+    made it (a routed call describes one expert of the stacks).  Returns (device, descriptor, `a` as a contiguous 2-D
+    tensor)."""
+    name = "grad_output" if transposed else "input"
+    device = _require_cuda(a, codes, codebooks, scales, bias, *extra)
+    _dtype_code(a)
+    if a.dtype != codebooks.dtype:
+        raise ValueError(f"{name} dtype {a.dtype} != codebooks dtype {codebooks.dtype}")
+    if w is None:
+        w = make_weight(codes, codebooks, scales.reshape(-1) if scales is not None else None, bias)
+    features = w.out_features if transposed else w.in_features
+    if a.shape[-1] != features:
+        raise ValueError(f"{name} has {a.shape[-1]} features, weight expects {features}")
+    flat = a.reshape(-1, a.shape[-1])
+    return device, w, flat if flat.is_contiguous() else flat.contiguous()
+
+
+def _segments(codebooks_stacked, n_seg: int, seg_rows):
+    """The C table of `seg_rows` (None stays None) for codebooks stacked as n_seg sets per linear."""
+    if not codebooks_stacked.is_contiguous() or (seg_rows is not None and len(seg_rows) != n_seg):
+        raise ValueError("codebooks must be a contiguous stack of one set per segment, matching seg_rows")
+    return None if seg_rows is None else (ctypes.c_int64 * n_seg)(*[int(r) for r in seg_rows])
+
+
+def _call(device, query: Optional[str], query_args, fn: str, args) -> bool:
+    """One library call that takes a workspace: `query(*query_args)` sizes it (no query or 0 bytes: none), then
+    `fn(*args, workspace, workspace_bytes, stream)` runs.  False when the library refuses the layout
+    (ERR_UNSUPPORTED); any other error raises."""
+    with _on_device(device):
+        L = _cabi.lib()
+        need = getattr(L, query)(*query_args) if query else 0
+        ws = _workspace(device, need) if need else None
+        rc = getattr(L, fn)(*args, *((ws.data_ptr(), ws.numel()) if ws is not None else (None, 0)), _stream_ptr(device))
+    if rc == _cabi.ERR_UNSUPPORTED:
+        return False
+    _cabi.check(rc)
+    return True
 
 
 def _call_matmat_ws(device, w, flat_input, flat_output, flags: int) -> None:
@@ -162,20 +189,16 @@ def _call_matmat_ws(device, w, flat_input, flat_output, flags: int) -> None:
 
 
 def _call_matmat_dequant_ex(device, w, flat_input, flat_output, flags: int) -> None:
-    batch = flat_input.shape[0]
-    with _on_device(device):
-        L = _cabi.lib()
-        need = L.aqlm_b200_matmat_dequant_workspace_bytes(ctypes.byref(w), batch) if batch > 0 else 0
-        ws = _workspace(device, need) if need else None
-        _cabi.check(L.aqlm_b200_matmat_dequant_ex(ctypes.byref(w), flat_input.data_ptr(), flat_output.data_ptr(), batch,
-                                                  flags, ws.data_ptr() if ws is not None else None,
-                                                  ws.numel() if ws is not None else 0, _stream_ptr(device)))
+    wp, batch = ctypes.byref(w), flat_input.shape[0]
+    if not _call(device, "aqlm_b200_matmat_dequant_workspace_bytes", (wp, batch), "aqlm_b200_matmat_dequant_ex",
+                 (wp, flat_input.data_ptr(), flat_output.data_ptr(), batch, flags)):
+        _cabi.check(_cabi.ERR_UNSUPPORTED)  # the entry itself runs the GEMV where the GEMM has no plan
 
 
 def matmat(input, codes, codebooks, scales, bias=None) -> torch.Tensor:
     """Fused gather + additive dequant + GEMV (+scale+bias), any scheme; for small batch (reference `*_matmat`).
     Batch-1 calls on 256-entry codebooks run the dot-product-LUT kernel."""
-    device, w, flat_input = _prepare(input, codes, codebooks, scales, bias)
+    device, w, flat_input = _operands(input, codes, codebooks, scales, bias)
     flat_output = torch.empty((flat_input.shape[0], w.out_features), dtype=input.dtype, device=device)
     _call_matmat_ws(device, w, flat_input, flat_output, 0)
     return flat_output.reshape(input.shape[:-1] + (w.out_features,))
@@ -183,7 +206,7 @@ def matmat(input, codes, codebooks, scales, bias=None) -> torch.Tensor:
 
 def matmat_dequant(input, codes, codebooks, scales, bias=None) -> torch.Tensor:
     """Fused dequant + wgmma tensor-core GEMM (+scale+bias); for large batch (reference `*_matmat_dequant`)."""
-    device, w, flat_input = _prepare(input, codes, codebooks, scales, bias)
+    device, w, flat_input = _operands(input, codes, codebooks, scales, bias)
     flat_output = torch.empty((flat_input.shape[0], w.out_features), dtype=input.dtype, device=device)
     _call_matmat_dequant_ex(device, w, flat_input, flat_output, 0)
     return flat_output.reshape(input.shape[:-1] + (w.out_features,))
@@ -214,44 +237,22 @@ def matmat_grouped(input, codes, codebooks_stacked, scales, bias, seg_rows, part
     return out.reshape(input.shape[:-1] + (w.out_features,))
 
 
-def _grouped_weight(codes, codebooks_stacked, scales, bias, seg_rows):
-    n_seg = codebooks_stacked.shape[0]
-    if n_seg != len(seg_rows) or not codebooks_stacked.is_contiguous():
-        raise ValueError("codebooks_stacked must be a contiguous [n_seg, ...] stack matching seg_rows")
-    w = make_weight(codes, codebooks_stacked[0], scales.reshape(-1) if scales is not None else None, bias)
-    return w, (ctypes.c_int64 * n_seg)(*[int(r) for r in seg_rows]), n_seg
-
-
 def matmat_dequant_grouped(input, codes, codebooks_stacked, scales, bias, seg_rows,
                            partial: bool = False) -> Optional[torch.Tensor]:
     """ONE wgmma GEMM launch for several linears sharing `input`, any batch and any scheme the GEMM covers: `codes`
     [sum(seg_rows), in/8, K] (row-concatenated), `codebooks_stacked` [n_seg, K, 2^nbits, 1, 8], `scales`/`bias`
     concatenated.  Returns [..., sum(seg_rows)] in the input dtype, or UNSCALED fp32 sums when `partial`.  Returns None
     when the library does not take the layout (ERR_UNSUPPORTED): the caller then runs the members."""
-    device = _require_cuda(input, codes, codebooks_stacked, scales, bias)
-    _dtype_code(input)
-    if input.dtype != codebooks_stacked.dtype:
-        raise ValueError(f"input dtype {input.dtype} != codebooks dtype {codebooks_stacked.dtype}")
-    w, seg, n_seg = _grouped_weight(codes, codebooks_stacked, None if partial else scales, None if partial else bias,
-                                    seg_rows)
-    if input.shape[-1] != w.in_features:
-        raise ValueError(f"input has {input.shape[-1]} features, weight expects {w.in_features}")
-    flat = input.reshape(-1, input.shape[-1])
-    if not flat.is_contiguous():
-        flat = flat.contiguous()
+    n_seg = codebooks_stacked.shape[0]
+    device, w, flat = _operands(input, codes, codebooks_stacked[0], None if partial else scales,
+                                None if partial else bias, extra=(scales, bias))
+    seg = _segments(codebooks_stacked, n_seg, seg_rows)
     batch = flat.shape[0]
     out = torch.empty((batch, w.out_features), dtype=torch.float32 if partial else input.dtype, device=device)
-    with _on_device(device):
-        L = _cabi.lib()
-        need = L.aqlm_b200_matmat_dequant_workspace_bytes(ctypes.byref(w), batch) if batch > 0 else 0
-        ws = _workspace(device, need) if need else None
-        rc = L.aqlm_b200_matmat_dequant_grouped(ctypes.byref(w), seg, n_seg, flat.data_ptr(), out.data_ptr(), batch,
-                                                _cabi.FLAG_PARTIAL_F32 if partial else 0,
-                                                ws.data_ptr() if ws is not None else None,
-                                                ws.numel() if ws is not None else 0, _stream_ptr(device))
-    if rc == _cabi.ERR_UNSUPPORTED:
+    wp = ctypes.byref(w)
+    if not _call(device, "aqlm_b200_matmat_dequant_workspace_bytes", (wp, batch), "aqlm_b200_matmat_dequant_grouped",
+                 (wp, seg, n_seg, flat.data_ptr(), out.data_ptr(), batch, _cabi.FLAG_PARTIAL_F32 if partial else 0)):
         return None
-    _cabi.check(rc)
     return out.reshape(input.shape[:-1] + (w.out_features,))
 
 
@@ -259,44 +260,46 @@ def matmat_dequant_transposed_grouped(grad_out, codes, codebooks_stacked, scales
     """Backward w.r.t. the input of a group in ONE transposed wgmma GEMM: grad_in = (grad_out * scales) @ W over the
     row-concatenated weight, `grad_out` [..., sum(seg_rows)] (the group's concatenated output gradient).  Returns None
     when the library does not take the layout (ERR_UNSUPPORTED)."""
-    device = _require_cuda(grad_out, codes, codebooks_stacked, scales)
-    _dtype_code(grad_out)
-    if grad_out.dtype != codebooks_stacked.dtype:
-        raise ValueError(f"grad_output dtype {grad_out.dtype} != codebooks dtype {codebooks_stacked.dtype}")
-    w, seg, n_seg = _grouped_weight(codes, codebooks_stacked, scales, None, seg_rows)
-    if grad_out.shape[-1] != w.out_features:
-        raise ValueError(f"grad_output has {grad_out.shape[-1]} features, weight has {w.out_features} output rows")
-    flat = grad_out.reshape(-1, grad_out.shape[-1])
-    if not flat.is_contiguous():
-        flat = flat.contiguous()
+    n_seg = codebooks_stacked.shape[0]
+    device, w, flat = _operands(grad_out, codes, codebooks_stacked[0], scales, None, transposed=True)
+    seg = _segments(codebooks_stacked, n_seg, seg_rows)
     batch = flat.shape[0]
     out = torch.empty((batch, w.in_features), dtype=grad_out.dtype, device=device)
-    with _on_device(device):
-        L = _cabi.lib()
-        need = L.aqlm_b200_matmat_dequant_transposed_workspace_bytes(ctypes.byref(w), batch) if batch > 0 else 0
-        ws = _workspace(device, need) if need else None
-        rc = L.aqlm_b200_matmat_dequant_transposed_grouped(ctypes.byref(w), seg, n_seg, flat.data_ptr(), out.data_ptr(),
-                                                           batch, ws.data_ptr() if ws is not None else None,
-                                                           ws.numel() if ws is not None else 0, _stream_ptr(device))
-    if rc == _cabi.ERR_UNSUPPORTED:
+    wp = ctypes.byref(w)
+    if not _call(device, "aqlm_b200_matmat_dequant_transposed_workspace_bytes", (wp, batch),
+                 "aqlm_b200_matmat_dequant_transposed_grouped", (wp, seg, n_seg, flat.data_ptr(), out.data_ptr(), batch)):
         return None
-    _cabi.check(rc)
     return out.reshape(grad_out.shape[:-1] + (w.in_features,))
 
 
 def _routed_weight(codes, codebooks_stacked, scales, seg_rows):
     """Descriptor of ONE expert whose pointers point at the stacks of all experts: codes [E, out, in/8, K], codebooks
-    [E, n_seg, K, 2^nbits, 1, 8], scales [E, out, ...]."""
+    [E, n_seg, K, 2^nbits, 1, 8], scales [E, out, ...]; with the seg table, n_seg and n_experts."""
     n_experts, n_seg = codebooks_stacked.shape[:2]
     if codes.dim() != 4 or codes.shape[0] != n_experts or codebooks_stacked.dim() != 6:
         raise ValueError("routed GEMM takes codes [E, out, in/8, K] and codebooks [E, n_seg, K, 2^nbits, 1, 8]")
-    if not codebooks_stacked.is_contiguous() or (seg_rows is not None and len(seg_rows) != n_seg):
-        raise ValueError("codebooks must be a contiguous [E, n_seg, ...] stack matching seg_rows")
+    seg = _segments(codebooks_stacked, n_seg, seg_rows)
     if scales.numel() != codes.shape[0] * codes.shape[1]:
         raise ValueError(f"scales have {scales.numel()} elements for {codes.shape[0]} experts of {codes.shape[1]} rows")
     w = make_weight(codes[0], codebooks_stacked[0, 0], scales.reshape(-1), None)
-    seg = None if seg_rows is None else (ctypes.c_int64 * n_seg)(*[int(r) for r in seg_rows])
     return w, seg, (n_seg if seg_rows is not None else 1), n_experts
+
+
+def _routed(a, codes, codebooks_stacked, scales, expert_offsets, seg_rows, transposed: bool):
+    """One routed GEMM (see matmat_dequant_routed): the descriptor is ONE expert's, its pointers point at the stacks."""
+    w, seg, n_seg, n_experts = _routed_weight(codes, codebooks_stacked, scales, seg_rows)
+    device, w, flat = _operands(a, codes, codebooks_stacked, scales, None, transposed, (expert_offsets,), w)
+    _check_offsets(expert_offsets, n_experts, device)
+    if a.dim() != 2:
+        raise ValueError(f"{'grad_output' if transposed else 'input'} must be [rows, features], got {tuple(a.shape)}")
+    rows = flat.shape[0]
+    out = torch.empty((rows, w.in_features if transposed else w.out_features), dtype=a.dtype, device=device)
+    wp = ctypes.byref(w)
+    fn = "aqlm_b200_matmat_dequant_transposed_routed" if transposed else "aqlm_b200_matmat_dequant_routed"
+    if not _call(device, "aqlm_b200_matmat_dequant_routed_workspace_bytes", (wp, n_experts, rows, int(transposed)), fn,
+                 (wp, seg, n_seg, n_experts, expert_offsets.data_ptr(), flat.data_ptr(), out.data_ptr(), rows)):
+        return None
+    return out
 
 
 def _check_offsets(expert_offsets, n_experts, device):
@@ -312,29 +315,7 @@ def matmat_dequant_routed(input, codes, codebooks_stacked, scales, expert_offset
     n_seg row-concatenated linears, None for one), `scales` [E, out, ...], `expert_offsets` int32 [E + 1] on the device
     (never read by the host: the call is graph-capturable).  Returns [rows, out] in the input dtype; rows outside
     [offsets[0], offsets[E]) are left unwritten.  Returns None when the library does not take the layout."""
-    device = _require_cuda(input, codes, codebooks_stacked, scales, expert_offsets)
-    _dtype_code(input)
-    if input.dtype != codebooks_stacked.dtype:
-        raise ValueError(f"input dtype {input.dtype} != codebooks dtype {codebooks_stacked.dtype}")
-    w, seg, n_seg, n_experts = _routed_weight(codes, codebooks_stacked, scales, seg_rows)
-    _check_offsets(expert_offsets, n_experts, device)
-    if input.dim() != 2 or input.shape[-1] != w.in_features:
-        raise ValueError(f"input must be [rows, {w.in_features}], got {tuple(input.shape)}")
-    flat = input if input.is_contiguous() else input.contiguous()
-    rows = flat.shape[0]
-    out = torch.empty((rows, w.out_features), dtype=input.dtype, device=device)
-    with _on_device(device):
-        L = _cabi.lib()
-        need = L.aqlm_b200_matmat_dequant_routed_workspace_bytes(ctypes.byref(w), n_experts, rows, 0) if rows else 0
-        ws = _workspace(device, need) if need else None
-        rc = L.aqlm_b200_matmat_dequant_routed(ctypes.byref(w), seg, n_seg, n_experts, expert_offsets.data_ptr(),
-                                               flat.data_ptr(), out.data_ptr(), rows,
-                                               ws.data_ptr() if ws is not None else None,
-                                               ws.numel() if ws is not None else 0, _stream_ptr(device))
-    if rc == _cabi.ERR_UNSUPPORTED:
-        return None
-    _cabi.check(rc)
-    return out
+    return _routed(input, codes, codebooks_stacked, scales, expert_offsets, seg_rows, False)
 
 
 def matmat_dequant_transposed_routed(grad_out, codes, codebooks_stacked, scales, expert_offsets,
@@ -342,29 +323,7 @@ def matmat_dequant_transposed_routed(grad_out, codes, codebooks_stacked, scales,
     """Backward w.r.t. the input of `matmat_dequant_routed` in ONE transposed wgmma GEMM launch: row r of grad_input is
     (grad_out[r] * scales_e) @ W_e for the expert e that owns row r.  Same arguments; rows outside [offsets[0],
     offsets[E]) are left unwritten.  Returns None when the library does not take the layout."""
-    device = _require_cuda(grad_out, codes, codebooks_stacked, scales, expert_offsets)
-    _dtype_code(grad_out)
-    if grad_out.dtype != codebooks_stacked.dtype:
-        raise ValueError(f"grad_output dtype {grad_out.dtype} != codebooks dtype {codebooks_stacked.dtype}")
-    w, seg, n_seg, n_experts = _routed_weight(codes, codebooks_stacked, scales, seg_rows)
-    _check_offsets(expert_offsets, n_experts, device)
-    if grad_out.dim() != 2 or grad_out.shape[-1] != w.out_features:
-        raise ValueError(f"grad_output must be [rows, {w.out_features}], got {tuple(grad_out.shape)}")
-    flat = grad_out if grad_out.is_contiguous() else grad_out.contiguous()
-    rows = flat.shape[0]
-    out = torch.empty((rows, w.in_features), dtype=grad_out.dtype, device=device)
-    with _on_device(device):
-        L = _cabi.lib()
-        need = L.aqlm_b200_matmat_dequant_routed_workspace_bytes(ctypes.byref(w), n_experts, rows, 1) if rows else 0
-        ws = _workspace(device, need) if need else None
-        rc = L.aqlm_b200_matmat_dequant_transposed_routed(ctypes.byref(w), seg, n_seg, n_experts,
-                                                          expert_offsets.data_ptr(), flat.data_ptr(), out.data_ptr(),
-                                                          rows, ws.data_ptr() if ws is not None else None,
-                                                          ws.numel() if ws is not None else 0, _stream_ptr(device))
-    if rc == _cabi.ERR_UNSUPPORTED:
-        return None
-    _cabi.check(rc)
-    return out
+    return _routed(grad_out, codes, codebooks_stacked, scales, expert_offsets, seg_rows, True)
 
 
 def _check_deterministic_codebook_grad() -> None:
@@ -407,38 +366,25 @@ def matmat_weight_grad(x, grad_y, codes, codebooks, scales, want_codebooks: bool
     either is None when not wanted.  Layouts the kernel refuses go through a dense formulation (dequant + matmul +
     index_add_).  The codebook gradient is not deterministic (atomic fp32 sums): under
     torch.use_deterministic_algorithms(True) requesting it raises (warns with warn_only=True)."""
-    device = _require_cuda(x, grad_y, codes, codebooks, scales)
-    _dtype_code(x)
-    if x.dtype != codebooks.dtype or grad_y.dtype != codebooks.dtype:
-        raise ValueError(f"input {x.dtype} / grad_output {grad_y.dtype} must match the codebooks' dtype {codebooks.dtype}")
+    device, w, flat_x = _operands(x, codes, codebooks, scales, None, extra=(grad_y,))
+    if grad_y.dtype != x.dtype or grad_y.shape[-1] != w.out_features or x.shape[:-1] != grad_y.shape[:-1]:
+        raise ValueError(f"grad_output {grad_y.dtype} {tuple(grad_y.shape)} does not match the input {x.dtype} "
+                         f"{tuple(x.shape)} of a {w.in_features} -> {w.out_features} linear")
     if want_codebooks:
         _check_deterministic_codebook_grad()
-    w = make_weight(codes, codebooks, scales.reshape(-1), None)
-    if x.shape[-1] != w.in_features or grad_y.shape[-1] != w.out_features or x.shape[:-1] != grad_y.shape[:-1]:
-        raise ValueError(f"input {tuple(x.shape)} / grad_output {tuple(grad_y.shape)} do not match a "
-                         f"{w.in_features} -> {w.out_features} linear")
-    flat_x = x.reshape(-1, w.in_features)
     flat_g = grad_y.reshape(-1, w.out_features)
-    flat_x = flat_x if flat_x.is_contiguous() else flat_x.contiguous()
     flat_g = flat_g if flat_g.is_contiguous() else flat_g.contiguous()
     batch = flat_x.shape[0]
     K, cb_size, _, g = codebooks.shape
     gcb = torch.zeros((K, cb_size, g), dtype=torch.float32, device=device) if want_codebooks else None
     gs = torch.zeros((w.out_features,), dtype=torch.float32, device=device) if want_scales else None
-    if batch > 0 and (want_codebooks or want_scales):
-        with _on_device(device):
-            L = _cabi.lib()
-            need = L.aqlm_b200_matmat_weight_grad_workspace_bytes(ctypes.byref(w), batch) if want_scales else 0
-            ws = _workspace(device, need) if need else None
-            rc = L.aqlm_b200_matmat_weight_grad(ctypes.byref(w), flat_x.data_ptr(), flat_g.data_ptr(), batch,
-                                                gcb.data_ptr() if gcb is not None else None,
-                                                gs.data_ptr() if gs is not None else None,
-                                                ws.data_ptr() if ws is not None else None,
-                                                ws.numel() if ws is not None else 0, _stream_ptr(device))
-        if rc == _cabi.ERR_UNSUPPORTED:
-            gcb, gs = _weight_grad_dense(flat_x, flat_g, codes, codebooks, scales, want_codebooks, want_scales)
-        else:
-            _cabi.check(rc)
+    wp = ctypes.byref(w)
+    if batch > 0 and (want_codebooks or want_scales) and not _call(
+            device, "aqlm_b200_matmat_weight_grad_workspace_bytes" if want_scales else None, (wp, batch),
+            "aqlm_b200_matmat_weight_grad", (wp, flat_x.data_ptr(), flat_g.data_ptr(), batch,
+                                             gcb.data_ptr() if gcb is not None else None,
+                                             gs.data_ptr() if gs is not None else None)):
+        gcb, gs = _weight_grad_dense(flat_x, flat_g, codes, codebooks, scales, want_codebooks, want_scales)
     return (None if gcb is None else gcb.reshape(codebooks.shape).to(codebooks.dtype),
             None if gs is None else gs.reshape(scales.shape).to(scales.dtype))
 
@@ -494,32 +440,16 @@ def matmat_dequant_transposed(input, codes, codebooks, scales, bias=None) -> tor
     Layouts the fused kernel does not cover (in_group_size 16, odd codebook counts) fall back to our dequant kernel +
     a dense matmul, as the reference does for every scheme.
     """
-    device = _require_cuda(input, codes, codebooks, scales)
-    _dtype_code(input)
-    if input.dtype != codebooks.dtype:
-        raise ValueError(f"grad_output dtype {input.dtype} != codebooks dtype {codebooks.dtype}")
-    w = make_weight(codes, codebooks, scales.reshape(-1), None)
-    if input.shape[-1] != w.out_features:
-        raise ValueError(f"grad_output has {input.shape[-1]} features, weight has {w.out_features} output rows")
-    flat = input.reshape(-1, input.shape[-1])
-    if not flat.is_contiguous():
-        flat = flat.contiguous()
+    device, w, flat = _operands(input, codes, codebooks, scales, None, transposed=True)
     batch = flat.shape[0]
     out = torch.empty((batch, w.in_features), dtype=input.dtype, device=device)
     if batch == 0:
         return out.reshape(input.shape[:-1] + (w.in_features,))
-    with _on_device(device):
-        L = _cabi.lib()
-        need = L.aqlm_b200_matmat_dequant_transposed_workspace_bytes(ctypes.byref(w), batch)
-        ws = _workspace(device, need) if need else None
-        rc = L.aqlm_b200_matmat_dequant_transposed(ctypes.byref(w), flat.data_ptr(), out.data_ptr(), batch,
-                                                   ws.data_ptr() if ws is not None else None,
-                                                   ws.numel() if ws is not None else 0, _stream_ptr(device))
-    if rc == _cabi.ERR_UNSUPPORTED:
+    wp = ctypes.byref(w)
+    if not _call(device, "aqlm_b200_matmat_dequant_transposed_workspace_bytes", (wp, batch),
+                 "aqlm_b200_matmat_dequant_transposed", (wp, flat.data_ptr(), out.data_ptr(), batch)):
         weight = dequant(codes, codebooks, None)  # unscaled [out, in]
         out = (flat * scales.reshape(1, -1)) @ weight
-    else:
-        _cabi.check(rc)
     return out.reshape(input.shape[:-1] + (w.in_features,))
 
 

@@ -89,7 +89,8 @@ int aqlm_b200_matmat_ws(const aqlm_b200_weight_t* w, const void* input, void* ou
 /* Grouped launch for several 1x16 linears that share the same input (q/k/v, gate/up): `w` describes the ROW-CONCATENATED
  * weights (codes [sum(seg_rows), in/8, 1], scales/bias [sum(seg_rows)]) and w->codebooks points to n_seg codebooks stacked
  * back to back (1 MiB each); output is [batch, sum(seg_rows)].  One launch instead of n_seg; batch <= 8.  New work (the
- * reference launches every linear separately); SURVEY §8f.2. */
+ * reference launches every linear separately); SURVEY §8f.2.  n_seg outside 1..4, an empty or negative segment, or rows
+ * that do not add up to out_features: AQLM_B200_ERR_SHAPE, before any device query, as for the grouped GEMMs below. */
 int aqlm_b200_matmat_grouped(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, const void* input,
                              void* output, int64_t batch, uint32_t flags, void* stream);
 

@@ -177,7 +177,7 @@ int main() {
       long long batch;
       int split;
       is >> batch >> di.sm_count >> split;
-      const GemmPlan p = op == "gemm" ? gemm_plan(w, batch, di, t, split != 0) : gemm_t_plan(w, batch, di, t, split != 0);
+      const GemmPlan p = gemm_plan(w, batch, op != "gemm", 0, di, t, split != 0);
       if (!p.ok) std::printf("0\n");
       else std::printf("1 %%d %%d %%d %%d %%d %%d %%d %%zu %%zu\n", p.tile_m, p.m_tiles, p.n_tiles, p.n_tile, p.ksplit, p.stages,
                        p.total_kblocks, p.counters_bytes, p.partials_bytes);

@@ -83,7 +83,7 @@ int main() {
     w.in_group_size = (int)g;
     w.out_group_size = 1;
     w.dtype = AQLM_B200_F16;
-    const GemmPlan p = gemm_routed_plan(w, rows, E, di, t, split != 0, transposed != 0);
+    const GemmPlan p = gemm_plan(w, rows, transposed != 0, E, di, t, split != 0);
     if (!p.ok) std::printf("0\n");
     else std::printf("1 %%d %%d %%d %%d %%d %%d %%d %%zu %%zu\n", p.tile_m, p.m_tiles, p.n_tiles, p.n_tile, p.ksplit, p.stages,
                      p.total_kblocks, p.counters_bytes, p.partials_bytes);
