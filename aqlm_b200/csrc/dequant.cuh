@@ -1,7 +1,9 @@
 // Materialise W [out_features, in_features] from codes/codebooks(/scales).
 // Replaces Code1x16Dequant / Code2x8Dequant / CodeKx8Dequant (reference cuda_kernel.cu:98-142, 235-294,
 // 392-468) and the `weight *= scales` launch behind code*_dequant (cuda_kernel.cpp:184-227): one thread
-// per weight group, additive sum in fp32, optional scale fused, one rounding, 16-byte coalesced stores.
+// per weight group, additive sum in fp32 (exact for codebook entries of one binade), optional scale fused as an fp32
+// multiply (rounded to fp32), then ONE rounding to T: W = rT(rf32(s * sum)), or rT(sum) without scales; 16-byte
+// coalesced stores.
 #pragma once
 
 #include "common.cuh"

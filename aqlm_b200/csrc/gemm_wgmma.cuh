@@ -449,6 +449,11 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
 #pragma unroll
             for (int k = 1; k < K; ++k) accum8<T>(gather(cb_vec(k, code_at(e * K + k))), f);
           }
+          // the transposed direction scales the fp32 sum here, so that it is rounded to T once
+          if constexpr (Dir::kScaleInProducer) {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) f[q] *= sc;
+          }
           wv[e][0].x = DT<T>::pack2(f[0], f[1]); wv[e][0].y = DT<T>::pack2(f[2], f[3]);
           wv[e][0].z = DT<T>::pack2(f[4], f[5]); wv[e][0].w = DT<T>::pack2(f[6], f[7]);
         }
@@ -470,9 +475,11 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         uint4 v = wv[e][0];
-        if constexpr (Dir::kScaleInProducer && K == 1) {
-          // one codebook: scale the packed vector with 4 packed multiplies (a 16-bit x 16-bit product is exact in fp32, so
-          // the packed multiply rounds exactly like fp32-multiply-then-round)
+        if constexpr (!INREG) {
+          // K >= 4: issue() wrote the finished vector (the fp32 sum, scaled in the transposed direction, rounded once)
+        } else if constexpr (Dir::kScaleInProducer && K == 1) {
+          // one codebook: scale the packed vector with 4 packed multiplies (the product of two fp16 or two bf16 values is
+          // exact in fp32, so the packed multiply's one rounding gives what fp32-multiply-then-round-to-T gives)
           if constexpr (DT<T>::is_bf16) {
             const __nv_bfloat162 s2 = __float2bfloat162_rn(sc);
             __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&v);

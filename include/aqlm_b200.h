@@ -69,6 +69,24 @@ uint64_t aqlm_b200_launch_count(void);
  * environment at run time call this to re-read them.  Not needed in normal use. */
 void aqlm_b200_reload_tunables(void);
 
+/* ---- Rounding ----------------------------------------------------------------------------------
+ * T is the weight's dtype (f16 or bf16); rT rounds to T and rf32 to fp32, both to nearest even.  Wsum = sum over the K
+ * codebooks of the selected entries, added in fp32 (exact whenever the entries of a group lie within 2^24 of each
+ * other's units); products and sums of the contraction accumulate in fp32.
+ *   GEMV and LUT kernels (aqlm_b200_matmat*, the batch passes behind aqlm_b200_matmat_dequant* for layouts the wgmma
+ *   kernel does not take, aqlm_b200_matmat_grouped, aqlm_b200_matmat_allreduce):
+ *       y = rT(rf32(sum_j x * Wsum * s + b))             W is never rounded
+ *   wgmma forward (aqlm_b200_matmat_dequant*, grouped, routed; any split):
+ *       y = rT(rf32(sum_j x * rT(Wsum) * s + b))          the tensor core takes W as a T operand
+ *   AQLM_B200_FLAG_PARTIAL_F32: the unscaled sum of the same products (GEMV: x * Wsum, wgmma: x * rT(Wsum)).
+ *   wgmma transposed (aqlm_b200_matmat_dequant_transposed*): grad_in = rT(sum_o g * rT(rf32(s * Wsum)))
+ *   aqlm_b200_dequant: rT(rf32(s * Wsum)), or rT(Wsum) without scales
+ *   aqlm_b200_scale_bias, aqlm_b200_allreduce_scale_bias: rT(rf32(p * s + b))
+ *   aqlm_b200_matmat_weight_grad: grad_scales from rT(Wsum), the operand the wgmma forward multiplies
+ * So for K >= 2 the two forward families differ by the rounding of W: the same row of the same layer can come out
+ * differently on either side of the GEMV / wgmma batch boundary.  For K = 1, Wsum is a codebook entry and both agree.
+ * Subnormal f16 scales, inputs and outputs are kept (no flush to zero); an f16 output past 65504 is +-inf. */
+
 /* ---- generic entry points -------------------------------------------------------------------- */
 
 /* Fused code-gather + additive dequant + GEMV with the scale/bias epilogue in the same launch.
