@@ -106,6 +106,12 @@ def lib():
                 L.aqlm_b200_matmat_weight_grad_workspace_bytes.argtypes = [wp, i64]
                 L.aqlm_b200_matmat_weight_grad_workspace_bytes.restype = ctypes.c_size_t
                 L.aqlm_b200_matmat_weight_grad.argtypes = [wp, vp, vp, i64, vp, vp, vp, ctypes.c_size_t, vp]
+                L.aqlm_b200_matmat_weight_grad_grouped.argtypes = [wp, ctypes.POINTER(i64), ctypes.c_int, vp, vp, i64, vp,
+                                                                  vp, vp, ctypes.c_size_t, vp]
+                L.aqlm_b200_matmat_weight_grad_routed_workspace_bytes.argtypes = [wp, ctypes.c_int, i64]
+                L.aqlm_b200_matmat_weight_grad_routed_workspace_bytes.restype = ctypes.c_size_t
+                L.aqlm_b200_matmat_weight_grad_routed.argtypes = [wp, ctypes.POINTER(i64), ctypes.c_int, ctypes.c_int, vp,
+                                                                 vp, vp, i64, vp, vp, vp, ctypes.c_size_t, vp]
                 L.aqlm_b200_scale_bias.argtypes = [vp, vp, vp, vp, i64, i64, i32, vp]
                 L.aqlm_b200_matmat_host.argtypes = [wp, vp, vp, vp, vp, i64, vp]
                 L.aqlm_b200_comm_shared_bytes.argtypes = [ctypes.c_int, i64]

@@ -584,8 +584,6 @@ static int run_gemm(const GemmCall& c, void* workspace, size_t workspace_bytes, 
   });
 }
 
-constexpr int kRoutedMaxExperts = 64;
-
 // Workspace of a GEMM call (n_experts > 0: routed) with split-K allowed: the plan's counters and partials when it
 // splits, else 0.  0 as well without a device, for a descriptor validate() refuses, rows <= 0 or too many experts.
 static size_t gemm_workspace_bytes(const aqlm_b200_weight_t* w, int64_t rows, bool transposed, int n_experts,
@@ -685,13 +683,44 @@ static int routed_gemm_checks(GemmCall& c, const int64_t* seg_rows) {
 }
 
 // ---- fused weight-gradient GEMM: host side ------------------------------------------------------------------------
-// Everything a weight-gradient call checks without a device: descriptor, pointers (ERR_SHAPE), then the layouts the
+// One weight-gradient call: plain (one segment, not routed), grouped (n_seg segments of the out rows) or routed
+// (n_experts > 0 stacked experts of w's shape, rows sorted by expert).
+struct WgradCall {
+  const aqlm_b200_weight_t* w;
+  const void *input, *grad_output;
+  int64_t rows;
+  float *grad_codebooks, *grad_scales;
+  int n_seg;
+  int seg_end[4];
+  const int32_t* expert_off;
+  int n_experts;
+};
+
+// Everything a weight-gradient call checks without a device: descriptor, segment table and expert count (grouped and
+// routed calls; seg_rows may be NULL for one segment of a routed call), pointers (ERR_SHAPE), then the layouts the
 // kernel takes (ERR_UNSUPPORTED): those of the transposed GEMM, whose grad_output operand it shares, and an aligned input.
-static int weight_grad_checks(const aqlm_b200_weight_t* w, const void* input, const void* grad_output, int64_t batch,
-                              const float* grad_codebooks, const float* grad_scales) {
+static int weight_grad_checks(WgradCall& c, const int64_t* seg_rows, bool grouped, bool routed) {
+  const aqlm_b200_weight_t* w = c.w;
+  const void *input = c.input, *grad_output = c.grad_output;
+  const int64_t batch = c.rows;
+  const float *grad_codebooks = c.grad_codebooks, *grad_scales = c.grad_scales;
   int rc = validate(w, grad_codebooks != nullptr);
   if (rc) return rc;
   if (batch < 0 || batch > 0x7fffffffll) return fail(AQLM_B200_ERR_SHAPE, "weight gradient: batch %lld out of range", (long long)batch);
+  if (grouped || routed) {
+    const int64_t one[1] = {w->out_features};
+    const int64_t* table = (seg_rows || c.n_seg != 1 || !routed) ? seg_rows : one;
+    if ((rc = segment_table(w, table, c.n_seg, routed ? "routed weight gradient" : "grouped weight gradient", c.seg_end)))
+      return rc;
+  }
+  if (routed) {
+    if (c.n_experts < 1 || c.n_experts > kRoutedMaxExperts)
+      return fail(AQLM_B200_ERR_SHAPE, "routed weight gradient takes 1..%d experts, got %d", kRoutedMaxExperts, c.n_experts);
+    if (w->out_features * c.n_experts > 0x7fffffffll)
+      return fail(AQLM_B200_ERR_SHAPE, "routed weight gradient: %d experts x %lld out rows exceed 2^31 - 1", c.n_experts,
+                  (long long)w->out_features);
+    if (!c.expert_off) return fail(AQLM_B200_ERR_SHAPE, "expert offsets pointer is NULL");
+  }
   if (!input || !grad_output) return fail(AQLM_B200_ERR_SHAPE, "weight gradient: input/grad_output pointer is NULL");
   if (!grad_codebooks && !grad_scales)
     return fail(AQLM_B200_ERR_SHAPE, "weight gradient: neither grad_codebooks nor grad_scales requested");
@@ -702,9 +731,14 @@ static int weight_grad_checks(const aqlm_b200_weight_t* w, const void* input, co
 }
 
 template <typename T, int K, int CB>
-static int launch_weight_grad(const aqlm_b200_weight_t* w, const void* input, const void* grad_output, int64_t batch,
-                              float* grad_codebooks, float* grad_scales, void* workspace, const WgradPlan& g,
-                              const DeviceInfo* di, cudaStream_t st) {
+static int launch_weight_grad(const WgradCall& c, void* workspace, const WgradPlan& g, const DeviceInfo* di,
+                              cudaStream_t st) {
+  const aqlm_b200_weight_t* w = c.w;
+  const void *input = c.input, *grad_output = c.grad_output;
+  const int64_t batch = c.rows;
+  float *grad_codebooks = c.grad_codebooks, *grad_scales = c.grad_scales;
+  const bool routed = c.n_experts > 0;
+  // a routed call's grad_output has the rows of one expert's out_features; the map spans every expert's codes below
   CUtensorMap tg, tx;
   if (int rc = encode_tmap(&tg, "grad_output", kTmapType<T>, grad_output, w->out_features, batch, w->out_features * 2, 64,
                            kWgradBlockK, CU_TENSOR_MAP_SWIZZLE_128B))
@@ -725,7 +759,34 @@ static int launch_weight_grad(const aqlm_b200_weight_t* w, const void* input, co
   p.nbits = w->nbits_per_codebook;
   p.total_kblocks = g.total_kblocks;
   p.stages = g.stages;
+  p.n_seg = c.n_seg;
+  for (int i = 0; i < 4; ++i) p.seg_end[i] = c.seg_end[i];
+  p.expert_off = c.expert_off;
+  p.n_experts = routed ? c.n_experts : 1;
+  p.rows = (int)batch;
+  if (routed)
+    return launch<gemm_wgrad_kernel<T, K, CB, true, true>>(di, dim3(g.out_tiles, g.in_tiles, c.n_experts), kWgradThreads,
+                                                           g.smem, st, 0, tg, tx, p);
+  if (c.n_seg > 1)
+    return launch<gemm_wgrad_kernel<T, K, CB, true>>(di, dim3(g.out_tiles, g.in_tiles), kWgradThreads, g.smem, st, 0, tg,
+                                                     tx, p);
   return launch<gemm_wgrad_kernel<T, K, CB>>(di, dim3(g.out_tiles, g.in_tiles), kWgradThreads, g.smem, st, 0, tg, tx, p);
+}
+
+// Everything a weight-gradient call does after its argument checks: plan on the current device, then one launch.
+static int run_weight_grad(const WgradCall& c, void* workspace, size_t workspace_bytes, void* stream) {
+  const DeviceInfo* di;
+  if (int rc = current_device(&di)) return rc;
+  const WgradPlan g = c.n_experts > 0 ? gemm_wgrad_routed_plan(*c.w, c.n_experts, c.rows, *di, tun())
+                                      : gemm_wgrad_plan(*c.w, c.rows, *di, tun());
+  if (!g.ok) return fail(AQLM_B200_ERR_UNSUPPORTED, "weight gradient: no wgmma plan for this descriptor and batch");
+  if (c.grad_scales && (!workspace || workspace_bytes < g.counters_bytes + g.dots_bytes))
+    return fail(AQLM_B200_ERR_SHAPE, "weight gradient: grad_scales needs a workspace of %zu bytes, got %zu",
+                g.counters_bytes + g.dots_bytes, workspace ? workspace_bytes : (size_t)0);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return with_gemm_scheme(c.w, [&](auto tag, auto K, auto CB) {
+    return launch_weight_grad<typename decltype(tag)::type, K, CB>(c, workspace, g, di, st);
+  });
 }
 
 }  // namespace aqlm_b200
@@ -963,20 +1024,39 @@ size_t aqlm_b200_matmat_weight_grad_workspace_bytes(const aqlm_b200_weight_t* w,
 int aqlm_b200_matmat_weight_grad(const aqlm_b200_weight_t* w, const void* input, const void* grad_output,
                                  int64_t batch, float* grad_codebooks, float* grad_scales, void* workspace,
                                  size_t workspace_bytes, void* stream) {
-  int rc = weight_grad_checks(w, input, grad_output, batch, grad_codebooks, grad_scales);
+  WgradCall c = {w, input, grad_output, batch, grad_codebooks, grad_scales, 1, {}, nullptr, 0};
+  int rc = weight_grad_checks(c, nullptr, false, false);
   if (rc || batch == 0) return rc;
-  const DeviceInfo* di;
-  if ((rc = current_device(&di))) return rc;
-  const WgradPlan g = gemm_wgrad_plan(*w, batch, *di, tun());
-  if (!g.ok) return fail(AQLM_B200_ERR_UNSUPPORTED, "weight gradient: no wgmma plan for this descriptor and batch");
-  if (grad_scales && (!workspace || workspace_bytes < g.counters_bytes + g.dots_bytes))
-    return fail(AQLM_B200_ERR_SHAPE, "weight gradient: grad_scales needs a workspace of %zu bytes, got %zu",
-                g.counters_bytes + g.dots_bytes, workspace ? workspace_bytes : (size_t)0);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return with_gemm_scheme(w, [&](auto tag, auto K, auto CB) {
-    return launch_weight_grad<typename decltype(tag)::type, K, CB>(w, input, grad_output, batch, grad_codebooks,
-                                                                   grad_scales, workspace, g, di, st);
-  });
+  const int out = (int)w->out_features;
+  for (int i = 0; i < 4; ++i) c.seg_end[i] = out;
+  return run_weight_grad(c, workspace, workspace_bytes, stream);
+}
+
+int aqlm_b200_matmat_weight_grad_grouped(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg,
+                                         const void* input, const void* grad_output, int64_t batch, float* grad_codebooks,
+                                         float* grad_scales, void* workspace, size_t workspace_bytes, void* stream) {
+  WgradCall c = {w, input, grad_output, batch, grad_codebooks, grad_scales, n_seg, {}, nullptr, 0};
+  int rc = weight_grad_checks(c, seg_rows, true, false);
+  if (rc || batch == 0) return rc;
+  return run_weight_grad(c, workspace, workspace_bytes, stream);
+}
+
+size_t aqlm_b200_matmat_weight_grad_routed_workspace_bytes(const aqlm_b200_weight_t* w, int n_experts, int64_t rows) {
+  if (validate(w, false) != AQLM_B200_OK || rows <= 0) return 0;
+  const DeviceInfo* di = device_info();
+  if (!di) return 0;
+  const WgradPlan g = gemm_wgrad_routed_plan(*w, n_experts, rows, *di, tun());
+  return g.ok ? g.counters_bytes + g.dots_bytes : 0;
+}
+
+int aqlm_b200_matmat_weight_grad_routed(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, int n_experts,
+                                        const int32_t* expert_offsets, const void* input, const void* grad_output,
+                                        int64_t rows, float* grad_codebooks, float* grad_scales, void* workspace,
+                                        size_t workspace_bytes, void* stream) {
+  WgradCall c = {w, input, grad_output, rows, grad_codebooks, grad_scales, n_seg, {}, expert_offsets, n_experts};
+  int rc = weight_grad_checks(c, seg_rows, false, true);
+  if (rc || rows == 0) return rc;
+  return run_weight_grad(c, workspace, workspace_bytes, stream);
 }
 
 int aqlm_b200_scale_bias(const float* partial, const void* scales, const void* bias, void* output, int64_t batch,

@@ -294,4 +294,18 @@ inline WgradPlan gemm_wgrad_plan(const aqlm_b200_weight_t& w, int64_t batch, con
   return g;
 }
 
+// The routed weight gradient of n_experts experts of w's shape over `rows` expert-sorted rows: grid (out_tiles,
+// in_tiles, E), one ticket word per (expert, out tile) -- E * out_tiles must fit the counter region -- and the row dots
+// [in_tiles][E * out].  Stages as the plain plan's (the k-block count of an expert is read on the device; total_kblocks
+// is the bound, all rows in one expert).
+inline WgradPlan gemm_wgrad_routed_plan(const aqlm_b200_weight_t& w, int n_experts, int64_t rows, const DeviceInfo& di,
+                                        const Tunables& t) {
+  WgradPlan g = gemm_wgrad_plan(w, rows, di, t);
+  if (!g.ok) return g;
+  if (n_experts < 1 || n_experts > kRoutedMaxExperts || (int64_t)n_experts * g.out_tiles > kGemmMaxTiles)
+    return WgradPlan();
+  g.dots_bytes *= (size_t)n_experts;
+  return g;
+}
+
 }  // namespace aqlm_b200

@@ -14,6 +14,8 @@
 
 namespace aqlm_b200 {
 
+constexpr int kRoutedMaxExperts = 64;  // experts of one routed call
+
 struct RoutedSlot {
   int expert;  // -1: the slot is past the last tile (the CTA has nothing to do)
   int row0;    // first input / output row of the slot's tile
@@ -42,6 +44,22 @@ __host__ __device__ inline RoutedSlot routed_slot(const int32_t* off, int n_expe
     lo = hi;
   }
   return RoutedSlot{-1, 0, 0};
+}
+
+// Expert e's effective rows [first, end) under the same clamping as routed_slot: the running maximum of the clamped
+// offsets, so end >= first and the ranges of the experts are disjoint and in expert order.
+struct RoutedRows {
+  int first, end;
+};
+__host__ __device__ inline RoutedRows routed_expert_rows(const int32_t* off, int rows, int e) {
+  auto clamp = [rows](int v) { return v < 0 ? 0 : (v > rows ? rows : v); };
+  int lo = clamp(off[0]);
+  for (int i = 1; i <= e; ++i) {
+    const int v = clamp(off[i]);
+    lo = v > lo ? v : lo;
+  }
+  const int hi = clamp(off[e + 1]);
+  return RoutedRows{lo, hi > lo ? hi : lo};
 }
 
 }  // namespace aqlm_b200

@@ -10,8 +10,10 @@ Which launch serves a call:
   * more rows, or an input that needs a gradient, for every scheme the wgmma GEMM covers (in_group 8, 8/16-bit codes,
     1/2/4/8 codebooks): the grouped GEMM over the row-concatenated weight (one launch), and for the gradient w.r.t. the
     input one grouped transposed GEMM (`_GroupedMatmul`);
-  * anything else -- up to 8 rows of other schemes, or a layout the library refuses -- the members one by one;
-  * so do calls that need a gradient w.r.t. a member's codebooks, scales or bias (no grouped weight-gradient kernel).
+  * anything else -- up to 8 rows of other schemes, or a layout the library refuses -- the members one by one.
+With trainable codebooks, scales or bias the same launch serves the forward, and the backward adds ONE grouped
+weight-gradient launch (`cuda_kernel.matmat_weight_grad_grouped`) whose stacked gradients are sliced onto the member
+parameters, which are what the optimizer and `state_dict` hold; the bias gradient is grad_y's column sums in fp32.
 """
 from __future__ import annotations
 
@@ -76,25 +78,72 @@ def _check_members(members) -> bool:
     return gemm_scheme(m0) and len(members) <= 4 and m0.codes.is_cuda
 
 
+def _member_params(members):
+    """The trainable parameters of every member, in the order _GroupedMatmul takes them: (codebooks, scales, bias) each."""
+    return [p for m in members for p in (m.codebooks, m.scales, m.bias)]
+
+
 class _GroupedMatmul(torch.autograd.Function):
     """Autograd node of a group's concatenated output y = [x W_1^T | x W_2^T | ...] (+ scales, bias).  `y` is what the
     group's forward kernel computed from `x` (the group has to know that the kernel took the layout before it builds this
-    node).  Only `x` receives a gradient, as in `_AqlmMatmul`: ONE grouped transposed GEMM over the concatenated weight,
-    or, for a layout it does not take, the members' own backward ops, summed."""
+    node).  `params` are the members' (codebooks, scales, bias) in member order (`_member_params`).  `x` gets ONE grouped
+    transposed GEMM over the concatenated weight, or, for a layout it does not take, the members' own backward ops,
+    summed.  The parameters that require a gradient get slices of ONE grouped weight-gradient launch (or, for a layout
+    it does not take, each member's own weight gradient); the others get None."""
 
     @staticmethod
-    def forward(ctx, x, y, group):
+    def forward(ctx, x, y, group, *params):
         ctx.group = group
+        # kept on ctx, not saved: the outputs are split per member, and each may be back-propagated on its own
+        ctx.x = x.detach() if any(ctx.needs_input_grad[3:]) else None
         return y
 
     @staticmethod
     def backward(ctx, grad_y):
-        from .inference_kernels import cuda_kernel
-
         g = ctx.group
-        gx = cuda_kernel.matmat_dequant_transposed_grouped(grad_y, g._fused_codes, g._fused_codebooks, g._fused_scales,
-                                                           g.seg_rows)
-        if gx is None:
+        gx = _grouped_input_grad(g, grad_y) if ctx.needs_input_grad[0] else None
+        grads = [None] * (3 * len(g.members))
+        if any(ctx.needs_input_grad[3:]):
+            grads = _grouped_weight_grads(g, ctx.x, grad_y, ctx.needs_input_grad[3:])
+        return (gx, None, None, *grads)
+
+
+def _grouped_weight_grads(g, x, grad_y, needs):
+    """Gradients of the members' (codebooks, scales, bias), flat in `_member_params` order, None where not needed."""
+    from .inference_kernels import cuda_kernel
+
+    want_cb, want_s = any(needs[0::3]), any(needs[1::3])
+    grad_y = grad_y.contiguous()
+    res = (None, None)
+    if want_cb or want_s:
+        res = cuda_kernel.matmat_weight_grad_grouped(x, grad_y, g._fused_codes, g._fused_codebooks, g._fused_scales,
+                                                     g.seg_rows, want_cb, want_s)
+    grads, off = [], 0
+    for i, m in enumerate(g.members):
+        n = m.out_features
+        gy = grad_y[..., off:off + n]
+        cb_i, s_i = None, None
+        if res is None:  # a layout the grouped kernel refuses: the member's own weight gradient
+            cb_i, s_i = cuda_kernel.matmat_weight_grad(x, gy.contiguous(), m.codes, m.codebooks, m.scales,
+                                                       needs[3 * i], needs[3 * i + 1])
+        else:
+            gcb, gs = res
+            cb_i = gcb[i] if gcb is not None and needs[3 * i] else None
+            s_i = gs[off:off + n] if gs is not None and needs[3 * i + 1] else None
+        b_i = None
+        if needs[3 * i + 2]:
+            b_i = gy.reshape(-1, n).sum(dim=0, dtype=torch.float32).to(m.bias.dtype)
+        grads += [cb_i if needs[3 * i] else None, s_i if needs[3 * i + 1] else None, b_i]
+        off += n
+    return grads
+
+
+def _grouped_input_grad(g, grad_y):
+    from .inference_kernels import cuda_kernel
+
+    gx = cuda_kernel.matmat_dequant_transposed_grouped(grad_y, g._fused_codes, g._fused_codebooks, g._fused_scales,
+                                                       g.seg_rows)
+    if gx is None:
             from .inference_kernels import get_backward_pass_kernel
 
             gx, off = None, 0
@@ -104,7 +153,7 @@ class _GroupedMatmul(torch.autograd.Function):
                                                                 m.codebooks, m.scales, m.bias)
                 gx = d if gx is None else gx + d
                 off += n
-        return gx, None, None
+    return gx
 
 
 class QuantizedLinearGroup(nn.Module):
@@ -122,14 +171,11 @@ class QuantizedLinearGroup(nn.Module):
 
     def forward(self, input: torch.Tensor) -> Tuple[torch.Tensor, ...]:
         rows = _rows(input)
-        # a gradient w.r.t. the input (LoRA / PEFT on frozen AQLM weights) goes through the grouped GEMM and its autograd
-        # node at any batch
-        needs_grad = torch.is_grad_enabled() and input.requires_grad
+        # a gradient w.r.t. the input (LoRA / PEFT on frozen AQLM weights) or the members' codebooks / scales / bias goes
+        # through the grouped GEMM and its autograd node at any batch
+        train_weights = torch.is_grad_enabled() and any(weights_require_grad(m) for m in self.members)
+        needs_grad = (torch.is_grad_enabled() and input.requires_grad) or train_weights
         if not self.fused or not input.is_cuda or rows < 1:
-            return tuple(m(input) for m in self.members)
-        if torch.is_grad_enabled() and any(weights_require_grad(m) for m in self.members):
-            # trainable codebooks / scales / bias: each member's own autograd node computes its weight gradients, which
-            # land on the member parameters (views into the fused storage)
             return tuple(m(input) for m in self.members)
         from .inference_kernels import cuda_kernel
 
@@ -151,7 +197,7 @@ class QuantizedLinearGroup(nn.Module):
         if y is None:
             return tuple(m(input) for m in self.members)
         if needs_grad:
-            y = _GroupedMatmul.apply(input, y, self)
+            y = _GroupedMatmul.apply(input, y, self, *_member_params(self.members))
         return tuple(torch.split(y, self.seg_rows, dim=-1))
 
 

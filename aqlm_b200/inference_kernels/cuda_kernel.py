@@ -389,6 +389,76 @@ def matmat_weight_grad(x, grad_y, codes, codebooks, scales, want_codebooks: bool
             None if gs is None else gs.reshape(scales.shape).to(scales.dtype))
 
 
+def _weight_grad_outputs(x, grad_y, out_features, codebooks_stacked, scales, want_codebooks, want_scales):
+    """Checks of a grouped or routed weight gradient and its zeroed fp32 outputs; the grad_output operand as a contiguous
+    2-D tensor."""
+    if grad_y.dtype != x.dtype or grad_y.shape[-1] != out_features or x.shape[:-1] != grad_y.shape[:-1]:
+        raise ValueError(f"grad_output {grad_y.dtype} {tuple(grad_y.shape)} does not match the input {x.dtype} "
+                         f"{tuple(x.shape)} of a linear with {out_features} out rows")
+    if want_codebooks:
+        _check_deterministic_codebook_grad()
+    flat_g = grad_y.reshape(-1, out_features)
+    flat_g = flat_g if flat_g.is_contiguous() else flat_g.contiguous()
+    dev = x.device
+    gcb = torch.zeros(codebooks_stacked.shape, dtype=torch.float32, device=dev) if want_codebooks else None
+    gs = torch.zeros((scales.numel(),), dtype=torch.float32, device=dev) if want_scales else None
+    return flat_g, gcb, gs
+
+
+def _weight_grad_result(gcb, gs, codebooks_stacked, scales):
+    return (None if gcb is None else gcb.to(codebooks_stacked.dtype),
+            None if gs is None else gs.reshape(scales.shape).to(scales.dtype))
+
+
+def matmat_weight_grad_grouped(x, grad_y, codes, codebooks_stacked, scales, seg_rows, want_codebooks: bool = True,
+                               want_scales: bool = True):
+    """`matmat_weight_grad` of a group of linears sharing `x` in ONE launch over the row-concatenated weight: `codes`
+    [sum(seg_rows), in/8, K], `codebooks_stacked` [n_seg, K, 2^nbits, 1, 8], `scales` [sum(seg_rows), ...], `grad_y`
+    [..., sum(seg_rows)] (the group's concatenated output gradient).  Returns (grad_codebooks [n_seg, ...] stacked like
+    the codebooks, grad_scales shaped like `scales`) in the parameters' dtypes, either None when not wanted; None when
+    the library does not take the layout.  The codebook gradient is not deterministic (see matmat_weight_grad)."""
+    n_seg = codebooks_stacked.shape[0]
+    device, w, flat_x = _operands(x, codes, codebooks_stacked[0], scales, None, extra=(grad_y,))
+    seg = _segments(codebooks_stacked, n_seg, seg_rows)
+    flat_g, gcb, gs = _weight_grad_outputs(x, grad_y, w.out_features, codebooks_stacked, scales, want_codebooks,
+                                           want_scales)
+    batch = flat_x.shape[0]
+    wp = ctypes.byref(w)
+    if batch > 0 and (want_codebooks or want_scales) and not _call(
+            device, "aqlm_b200_matmat_weight_grad_workspace_bytes" if want_scales else None, (wp, batch),
+            "aqlm_b200_matmat_weight_grad_grouped", (wp, seg, n_seg, flat_x.data_ptr(), flat_g.data_ptr(), batch,
+                                                     gcb.data_ptr() if gcb is not None else None,
+                                                     gs.data_ptr() if gs is not None else None)):
+        return None
+    return _weight_grad_result(gcb, gs, codebooks_stacked, scales)
+
+
+def matmat_weight_grad_routed(x, grad_y, codes, codebooks_stacked, scales, expert_offsets, seg_rows=None,
+                              want_codebooks: bool = True, want_scales: bool = True):
+    """The weight gradient of `matmat_dequant_routed` in ONE launch over all experts: `x` [rows, in] and `grad_y` [rows,
+    out] sorted by expert, the stacks and `expert_offsets` as for matmat_dequant_routed.  Expert e's gradients contract
+    over its own rows only; rows outside every expert contribute nothing, whatever they hold.  Returns (grad_codebooks
+    [E, n_seg, K, 2^nbits, 1, 8], grad_scales shaped like `scales`) in the parameters' dtypes, either None when not
+    wanted; an expert without rows gets zeros.  None when the library does not take the layout.  Graph-capturable: the
+    host never reads the offsets."""
+    w, seg, n_seg, n_experts = _routed_weight(codes, codebooks_stacked, scales, seg_rows)
+    device, w, flat_x = _operands(x, codes, codebooks_stacked, scales, None, False, (grad_y, expert_offsets), w)
+    _check_offsets(expert_offsets, n_experts, device)
+    if x.dim() != 2:
+        raise ValueError(f"input must be [rows, features], got {tuple(x.shape)}")
+    flat_g, gcb, gs = _weight_grad_outputs(x, grad_y, w.out_features, codebooks_stacked, scales, want_codebooks,
+                                           want_scales)
+    rows = flat_x.shape[0]
+    wp = ctypes.byref(w)
+    if rows > 0 and (want_codebooks or want_scales) and not _call(
+            device, "aqlm_b200_matmat_weight_grad_routed_workspace_bytes" if want_scales else None,
+            (wp, n_experts, rows), "aqlm_b200_matmat_weight_grad_routed",
+            (wp, seg, n_seg, n_experts, expert_offsets.data_ptr(), flat_x.data_ptr(), flat_g.data_ptr(), rows,
+             gcb.data_ptr() if gcb is not None else None, gs.data_ptr() if gs is not None else None)):
+        return None
+    return _weight_grad_result(gcb, gs, codebooks_stacked, scales)
+
+
 def matmat_partial(input, codes, codebooks) -> torch.Tensor:
     """UNSCALED fp32 partial products [batch, out] of an in_features shard (to be all-reduced).  Above GEMV_MAX_ROWS
     rows (prefill) this is the wgmma GEMM, as in QuantizedLinear; below, the GEMV / LUT kernels."""

@@ -14,9 +14,13 @@ all experts:
   * the combine sum_j w[t, j] * y[pair(t, j)], in fp32 in slot order, rounded once to the activation dtype.
 
 Nothing reads the routing on the host, so a decode step can be captured in a CUDA graph and replayed with new routing.
-Gradients flow to `hidden_states` (one routed transposed GEMM per projection) and to `top_k_weights` (ordinary
-autograd); the quantized weights are frozen.  A scheme the routed GEMM does not take (e.g. in_group 16) runs the
-transformers algorithm over the member `QuantizedLinear`s: correct, but it syncs with the host and is not capturable.
+Gradients flow to `hidden_states` (one routed transposed GEMM per projection), to `top_k_weights` (ordinary autograd)
+and, once unfrozen, to the members' codebooks and scales: one routed weight-gradient launch per projection over all
+experts, whose stacked gradients are sliced onto the member parameters.  Every expert's trainable parameters then
+receive a gradient, ZERO for an expert that got no tokens (as transformers' dense `MixtralExperts`, whose experts are
+one 3-D parameter, gives), so a training step stays free of host syncs and capturable too.  A scheme the routed GEMM
+does not take (e.g. in_group 16) runs the transformers algorithm over the member `QuantizedLinear`s: correct, but it
+syncs with the host, is not capturable, and leaves the gradients of experts without tokens None.
 
 The member parameters are views into stacked per-projection buffers (as `grouped._fuse_storage` does for a group); the
 stacks are rebuilt whenever the module is moved or cast (`_apply`) or after a load that replaced the parameters.
@@ -29,7 +33,7 @@ import torch
 from torch import nn
 
 from .grouped import gemm_scheme
-from .inference import QuantizedLinear, weights_require_grad
+from .inference import QuantizedLinear
 
 
 def route(top_k_index: torch.Tensor, n_experts: int) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
@@ -49,26 +53,52 @@ def route(top_k_index: torch.Tensor, n_experts: int) -> Tuple[torch.Tensor, torc
 
 class _RoutedMatmul(torch.autograd.Function):
     """Autograd node of a routed projection y = routed(x; stacked weights).  `y` is what the routed forward kernel
-    computed from `x`; the backward is one routed transposed GEMM.  Rows that belong to no expert (dropped pairs, at the
-    end of the sorted rows) are never written by the kernels; their input gradient is set to zero here."""
+    computed from `x`; `params` are the projection's member (codebooks, scales) pairs, expert-major and, within an
+    expert, in segment order (w1, w3 for the gate/up projection).  The input gradient is one routed transposed GEMM;
+    rows that belong to no expert (dropped pairs, at the end of the sorted rows) are never written by the kernels, and
+    their input gradient is set to zero here.  The parameters that require a gradient get slices of ONE routed
+    weight-gradient launch over the sorted rows (zero for an expert without rows); the others get None."""
 
     @staticmethod
-    def forward(ctx, x, y, weights, offsets, row_valid):
+    def forward(ctx, x, y, weights, offsets, row_valid, *params):
         ctx.weights, ctx.row_valid = weights, row_valid
-        ctx.save_for_backward(offsets)
+        ctx.save_for_backward(offsets, x if any(ctx.needs_input_grad[5:]) else None)
         return y
 
     @staticmethod
     def backward(ctx, grad_y):
         from .inference_kernels import cuda_kernel
 
-        (offsets,) = ctx.saved_tensors
+        offsets, x = ctx.saved_tensors
         codes, codebooks, scales, seg_rows = ctx.weights
-        gx = cuda_kernel.matmat_dequant_transposed_routed(grad_y.contiguous(), codes, codebooks, scales, offsets, seg_rows)
-        if gx is None:
-            raise NotImplementedError("the routed transposed GEMM refused a layout its forward took")
-        return torch.where(ctx.row_valid[:, None], gx, torch.zeros((), dtype=gx.dtype, device=gx.device)), None, None, \
-            None, None
+        grad_y = grad_y.contiguous()
+        gx = None
+        if ctx.needs_input_grad[0]:
+            gx = cuda_kernel.matmat_dequant_transposed_routed(grad_y, codes, codebooks, scales, offsets, seg_rows)
+            if gx is None:
+                raise NotImplementedError("the routed transposed GEMM refused a layout its forward took")
+            gx = torch.where(ctx.row_valid[:, None], gx, torch.zeros((), dtype=gx.dtype, device=gx.device))
+        needs = ctx.needs_input_grad[5:]
+        grads = [None] * len(needs)
+        want_cb, want_s = any(needs[0::2]), any(needs[1::2])
+        if want_cb or want_s:
+            res = cuda_kernel.matmat_weight_grad_routed(x, grad_y, codes, codebooks, scales, offsets, seg_rows, want_cb,
+                                                        want_s)
+            if res is None:
+                raise NotImplementedError("the routed weight gradient refused a layout the routed GEMM took")
+            gcb, gs = res
+            E, n_seg = codebooks.shape[:2]
+            rows = seg_rows if seg_rows is not None else [codes.shape[1]]
+            for e in range(E):
+                off = 0
+                for i, n in enumerate(rows):
+                    j = 2 * (e * n_seg + i)
+                    if needs[j]:
+                        grads[j] = gcb[e, i]
+                    if needs[j + 1]:
+                        grads[j + 1] = gs[e, off:off + n]
+                    off += n
+        return (gx, None, None, None, None, *grads)
 
 
 class _Expert(nn.Module):
@@ -129,35 +159,38 @@ class QuantizedMixtralExperts(nn.Module):
 
     # -- forward ------------------------------------------------------------------------------------------------------
     def forward(self, hidden_states: torch.Tensor, top_k_index: torch.Tensor, top_k_weights: torch.Tensor) -> torch.Tensor:
-        # trainable codebooks / scales: the members' own autograd nodes (no routed weight-gradient kernel)
-        train_weights = torch.is_grad_enabled() and any(weights_require_grad(m) for m in self.modules()
-                                                        if isinstance(m, QuantizedLinear))
-        if self.routed and hidden_states.is_cuda and not train_weights:
+        if self.routed and hidden_states.is_cuda:
             out = self._forward_routed(hidden_states, top_k_index, top_k_weights)
             if out is not None:
                 return out
         return self._forward_loop(hidden_states, top_k_index, top_k_weights)
 
-    def _project(self, x, weights, offsets, row_valid):
+    def _params(self, names) -> list:
+        """The (codebooks, scales) of the members `names` of every expert, in the order _RoutedMatmul takes them."""
+        return [p for e in range(self.num_experts) for n in names
+                for p in (getattr(self.expert(e), n).codebooks, getattr(self.expert(e), n).scales)]
+
+    def _project(self, x, weights, offsets, row_valid, params):
         from .inference_kernels import cuda_kernel
 
         codes, codebooks, scales, seg_rows = weights
         y = cuda_kernel.matmat_dequant_routed(x.detach(), codes, codebooks, scales, offsets, seg_rows)
-        if y is None or not (torch.is_grad_enabled() and x.requires_grad):
+        # the node is built whenever a weight is trainable, even if x needs no gradient
+        if y is None or not (torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params))):
             return y
-        return _RoutedMatmul.apply(x, y, weights, offsets, row_valid)
+        return _RoutedMatmul.apply(x, y, weights, offsets, row_valid, *params)
 
     def _forward_routed(self, hidden_states, top_k_index, top_k_weights) -> Optional[torch.Tensor]:
         T, k = top_k_index.shape
         order, offsets, valid = route(top_k_index, self.num_experts)
         row_valid = valid[order]  # per sorted row: the valid pairs come first
         xs = hidden_states.index_select(0, order // k)
-        gu = self._project(xs, self._w13, offsets, row_valid)
+        gu = self._project(xs, self._w13, offsets, row_valid, self._params(("w1", "w3")))
         if gu is None:
             return None
         gate, up = gu.split(self.intermediate_dim, dim=-1)
         h = self.act_fn(gate) * up
-        ys = self._project(h, self._w2, offsets, row_valid)
+        ys = self._project(h, self._w2, offsets, row_valid, self._params(("w2",)))
         if ys is None:
             return None
         # back to (token, slot) order; rows of dropped pairs hold whatever the kernels left there: masked, not scaled

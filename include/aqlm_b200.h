@@ -211,6 +211,36 @@ int aqlm_b200_matmat_weight_grad(const aqlm_b200_weight_t* w, const void* input,
                                  int64_t batch, float* grad_codebooks, float* grad_scales, void* workspace,
                                  size_t workspace_bytes, void* stream);
 
+/* Grouped weight gradient: the gradients of n_seg linears that share their input, in ONE launch over the
+ * row-concatenated weight.  `w`, `seg_rows` and `n_seg` describe the group as for aqlm_b200_matmat_dequant_grouped
+ * (codes and scales [sum(seg_rows)], w->codebooks points to n_seg codebook sets back to back).  grad_codebooks is fp32
+ * [n_seg][K][2^nbits][8], segment i's gradient in slice i, and is ADDED into; grad_scales is fp32 [sum(seg_rows)] and is
+ * WRITTEN.  The workspace is aqlm_b200_matmat_weight_grad_workspace_bytes of the concatenated descriptor.  Determinism,
+ * NULL outputs, errors and launches as for aqlm_b200_matmat_weight_grad; in addition n_seg outside 1..4, an empty
+ * segment, or rows that do not add up to out_features return AQLM_B200_ERR_SHAPE before any device query. */
+int aqlm_b200_matmat_weight_grad_grouped(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg,
+                                         const void* input, const void* grad_output, int64_t batch, float* grad_codebooks,
+                                         float* grad_scales, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Routed weight gradient, the backward of aqlm_b200_matmat_dequant_routed w.r.t. the experts' codebooks and scales, in
+ * ONE launch over all experts.  `w`, `seg_rows`, `n_seg`, `n_experts` and the device array `expert_offsets` as for the
+ * routed GEMMs (seg_rows == NULL with n_seg == 1: one segment; offsets clamped and made non-decreasing, never read by
+ * the host, so the call is capturable).  input [rows, in] and grad_output [rows, out] are sorted by expert; expert e's
+ * gradients contract over its own rows only, and rows outside every expert contribute nothing even if they hold NaN or
+ * inf.  grad_codebooks is fp32 [E][n_seg][K][2^nbits][8] and is ADDED into; grad_scales is fp32 [E][out] and is WRITTEN,
+ * including 0 for an expert without rows (whose grad_codebooks slice is left untouched).  The workspace comes from
+ * aqlm_b200_matmat_weight_grad_routed_workspace_bytes (counters, left at zero, and row dots [in_tiles][E * out]);
+ * n_experts * ceil(out / 128) above 8192 has no plan (AQLM_B200_ERR_UNSUPPORTED).  grad_scales is deterministic (per
+ * expert and out tile the row dots are added in a fixed order); grad_codebooks is summed in atomic arrival order.
+ * Errors, before any device query: AQLM_B200_ERR_SHAPE as for the routed GEMMs and for both outputs NULL;
+ * AQLM_B200_ERR_UNSUPPORTED for the layouts aqlm_b200_matmat_weight_grad refuses.  rows == 0: OK, no launch; exactly
+ * one launch otherwise. */
+size_t aqlm_b200_matmat_weight_grad_routed_workspace_bytes(const aqlm_b200_weight_t* w, int n_experts, int64_t rows);
+int aqlm_b200_matmat_weight_grad_routed(const aqlm_b200_weight_t* w, const int64_t* seg_rows, int n_seg, int n_experts,
+                                        const int32_t* expert_offsets, const void* input, const void* grad_output,
+                                        int64_t rows, float* grad_codebooks, float* grad_scales, void* workspace,
+                                        size_t workspace_bytes, void* stream);
+
 /* Epilogue of the sharded path: output[b,o] = (T)(partial[b,o] * scales[o] + bias[o]) after the
  * all-reduce of the fp32 partials (new work; the reference has no multi-GPU hot path, SURVEY §8e). */
 int aqlm_b200_scale_bias(const float* partial, const void* scales, const void* bias, void* output, int64_t batch,
