@@ -23,9 +23,9 @@ const DeviceInfo* device_info() {
     return nullptr;
   }
   DeviceInfo& d = infos[dev];
-  if (!d.ok) {
+  if (!d.ok.load(std::memory_order_acquire)) {
     std::lock_guard<std::mutex> lock(mu);
-    if (!d.ok) {
+    if (!d.ok.load(std::memory_order_relaxed)) {
       cudaError_t e = cudaDeviceGetAttribute(&d.sm_count, cudaDevAttrMultiProcessorCount, dev);
       if (e == cudaSuccess) e = cudaDeviceGetAttribute(&d.cc_major, cudaDevAttrComputeCapabilityMajor, dev);
       if (e == cudaSuccess) e = cudaDeviceGetAttribute(&d.cc_minor, cudaDevAttrComputeCapabilityMinor, dev);
@@ -35,7 +35,7 @@ const DeviceInfo* device_info() {
         return nullptr;
       }
       d.index = dev;
-      d.ok = true;
+      d.ok.store(true, std::memory_order_release);
     }
   }
   if (d.cc_major != 9 || d.cc_minor != 0) {
@@ -137,15 +137,19 @@ static int with_n_tile(int n_tile, F&& f) {
 // ---- launches -------------------------------------------------------------------------------------------------
 // Opt-in dynamic shared memory.  cudaFuncSetAttribute applies to the CURRENT device only, so the high-water mark is
 // kept per (kernel instantiation, device): a process that drives several GPUs configures each of them.  The marks are
-// keyed on the kernel itself, not on its type: several kernels share one function-pointer type.
+// keyed on the kernel itself, not on its type: several kernels share one function-pointer type.  The attribute only
+// ever rises: host threads that launch the same kernel with different sizes raise it under one lock, so no thread can
+// set it below a size another thread's launch, or the stored mark, relies on.
 template <auto Kernel>
 static int ensure_smem(size_t smem, const DeviceInfo* di) {
   static std::atomic<size_t> marks[kMaxDevices];
+  static std::mutex mu;
   std::atomic<size_t>& m = marks[di->index];
-  if (smem > 48 * 1024 && m.load(std::memory_order_relaxed) < smem) {
-    AQLM_CUDA_CHECK(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    m.store(smem, std::memory_order_relaxed);
-  }
+  if (smem <= 48 * 1024 || m.load(std::memory_order_acquire) >= smem) return AQLM_B200_OK;
+  std::lock_guard<std::mutex> lock(mu);
+  if (m.load(std::memory_order_relaxed) >= smem) return AQLM_B200_OK;
+  AQLM_CUDA_CHECK(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  m.store(smem, std::memory_order_release);
   return AQLM_B200_OK;
 }
 

@@ -47,7 +47,8 @@ struct DeviceInfo {
   int sm_count = 0;
   int cc_major = 0, cc_minor = 0;
   int max_smem_optin = 0;
-  bool ok = false;
+  // Set (release) after the fields above are written; a reader that sees it (acquire) sees them too.
+  std::atomic<bool> ok{false};
 };
 const DeviceInfo* device_info();  // for the current device; nullptr on failure (error set)
 

@@ -8,6 +8,18 @@
  * kept between calls (reference ownership model, cuda_kernel.cpp:159-163).  All launches go to the
  * stream given and are CUDA-graph capturable.
  *
+ * Programmatic dependent launch (AQLM_B200_PDL=1, the default): some kernels read weights in their prologue, BEFORE
+ * their dependency wait.  The wgmma GEMMs (forward and transposed) read code tiles, codebook entries and scales there;
+ * the GEMVs and the LUT GEMVs read codes and codebooks there, and scales and bias after the wait.  Weights written by
+ * the immediately preceding kernel in the stream (an optimizer step, a dtype conversion, a fusion copy) are therefore
+ * read before that kernel is known to be complete.  tests/test_zz_ordering.py launches each of these entry points
+ * right behind an in-place kernel that rewrote one of its operands, with PDL on and off, and checks every output
+ * exactly; it shows what was observed on the hardware it ran on, not a guarantee of the programming model.
+ * Activations, expert offsets, workspaces and outputs are touched only after the wait.
+ *
+ * Host threads: the per-device queries and the per-kernel shared-memory attributes are set up under locks, so calls
+ * may come from several host threads at once.  Calls that may run concurrently must not share a workspace.
+ *
  * Reference citations are relative to /root/reference/inference_lib/src/aqlm/inference_kernels/.
  *
  * Tensor layouts (identical to the reference module, inference.py:39-61):
