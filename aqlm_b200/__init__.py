@@ -14,6 +14,7 @@ from .inference_kernels import cuda_kernel as _cuda_kernel  # noqa: F401  (regis
 
 from .grouped import QuantizedLinearGroup, ShardedQuantizedLinearGroup  # noqa: E402,F401
 from .hf import fuse_shared_input_linears  # noqa: E402,F401
+from .lora import LoraQuantizedLinear, add_lora, load_lora_adapter, save_lora_adapter  # noqa: E402,F401
 
 __version__ = "1.1.6+b200.1"  # tracks the reference's aqlm 1.1.6 (inference_lib/setup.cfg:2-3); same string in pyproject.toml
 

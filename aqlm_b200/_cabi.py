@@ -22,7 +22,7 @@ NVCC_FLAGS = [
 ]
 
 OK, ERR_DTYPE, ERR_UNSUPPORTED, ERR_SHAPE, ERR_CUDA, ERR_ARCH = range(6)
-F16, BF16 = 0, 1
+F16, BF16, F32 = 0, 1, 2
 FLAG_PARTIAL_F32 = 1
 
 
@@ -34,6 +34,12 @@ class Weight(ctypes.Structure):
         ("num_codebooks", ctypes.c_int32), ("nbits_per_codebook", ctypes.c_int32), ("in_group_size", ctypes.c_int32),
         ("out_group_size", ctypes.c_int32), ("dtype", ctypes.c_int32), ("reserved", ctypes.c_int32),
     ]
+
+
+class Lora(ctypes.Structure):
+    """aqlm_b200_lora_t"""
+    _fields_ = [("down", ctypes.c_void_p), ("up", ctypes.c_void_p), ("rank", ctypes.c_int32), ("dtype", ctypes.c_int32),
+                ("scaling", ctypes.c_float)]
 
 
 _lib = None
@@ -112,6 +118,10 @@ def lib():
                 L.aqlm_b200_matmat_weight_grad_routed_workspace_bytes.restype = ctypes.c_size_t
                 L.aqlm_b200_matmat_weight_grad_routed.argtypes = [wp, ctypes.POINTER(i64), ctypes.c_int, ctypes.c_int, vp,
                                                                  vp, vp, i64, vp, vp, vp, ctypes.c_size_t, vp]
+                lp = ctypes.POINTER(Lora)
+                L.aqlm_b200_matmat_lora.argtypes = [wp, lp, vp, vp, vp, i64, vp]
+                L.aqlm_b200_matmat_dequant_lora.argtypes = [wp, lp, vp, vp, vp, i64, vp, ctypes.c_size_t, vp]
+                L.aqlm_b200_matmat_dequant_transposed_lora.argtypes = [wp, lp, vp, vp, vp, i64, vp, ctypes.c_size_t, vp]
                 L.aqlm_b200_scale_bias.argtypes = [vp, vp, vp, vp, i64, i64, i32, vp]
                 L.aqlm_b200_matmat_host.argtypes = [wp, vp, vp, vp, vp, i64, vp]
                 L.aqlm_b200_comm_shared_bytes.argtypes = [ctypes.c_int, i64]

@@ -505,7 +505,15 @@ struct GemmCall {
   int seg_end[4];
   const int32_t* expert_off;
   int n_experts;
+  // a plain call with a LoRA adapter (NULL: none): lora_in is U [rows][rank] forward, V [rows][rank] transposed
+  const aqlm_b200_lora_t* lora;
+  const void* lora_in;
 };
+
+// The adapter of a validated call as the kernels take it: the up-projection B forward, the down-projection A transposed
+static LoraArgs lora_args(const aqlm_b200_lora_t* lora, const void* lora_in, bool transposed) {
+  return {lora_in, transposed ? lora->down : lora->up, lora->rank, lora->dtype == AQLM_B200_F32 ? 1 : 0, lora->scaling};
+}
 
 // A call on one validated plain linear: one segment, not routed.
 static GemmCall plain_gemm_call(const aqlm_b200_weight_t* w, const void* b, void* y, int64_t rows, bool transposed,
@@ -554,7 +562,15 @@ static int launch_gemm(const GemmCall& c, const GemmPlan& g, void* workspace, co
   p.n_experts = n_experts;
   return with_n_tile(g.n_tile, [&](auto N) {
     const dim3 grid(g.m_tiles, g.ksplit, g.n_tiles);  // routed: n_tiles is the slot count
-    const size_t smem = gemm_smem_layout(g.stages, N, Dir::kCtileBytes).total;
+    const GemmSmem layout = gemm_smem_layout(g.stages, N, Dir::kCtileBytes);
+    const size_t smem = layout.total;
+    if (c.lora) {
+      // the adapter's term is staged below the barriers; two stages of any N already hold it (never refused in practice)
+      if (gemm_lora_smem_bytes(c.lora->rank, N) > layout.full)
+        return fail(AQLM_B200_ERR_UNSUPPORTED, "LoRA GEMM: the adapter tile does not fit the plan's stage buffers");
+      constexpr auto kernel = TRANSPOSED ? gemm_dequant_t_lora_kernel<T, K, CB, N> : gemm_dequant_lora_kernel<T, K, CB, N>;
+      return launch<kernel>(di, grid, kGemmThreads, smem, st, 0, tb, tc, p, lora_args(c.lora, c.lora_in, TRANSPOSED));
+    }
     if (c.n_experts > 0) {
       constexpr auto kernel = TRANSPOSED ? gemm_dequant_t_routed_kernel<T, K, CB, N> : gemm_dequant_routed_kernel<T, K, CB, N>;
       return launch<kernel>(di, grid, kGemmThreads, smem, st, 0, tb, tc, p);
@@ -684,6 +700,45 @@ static int routed_gemm_checks(GemmCall& c, const int64_t* seg_rows) {
   if (!c.expert_off) return fail(AQLM_B200_ERR_SHAPE, "expert offsets pointer is NULL");
   if (!c.b || !c.y) return fail(AQLM_B200_ERR_SHAPE, "input/output pointer is NULL");
   return gemm_layout_checks(w, c.b, c.transposed, "routed GEMM");
+}
+
+// ---- LoRA adapters on plain linears: argument checks --------------------------------------------------------------
+// Everything an adapter call checks without a device, in this order: descriptor, batch and pointers (ERR_SHAPE), the
+// adapter (ERR_SHAPE for NULL pointers, ERR_UNSUPPORTED for a rank outside 8..64 or not a multiple of 8, ERR_DTYPE for
+// operands that are neither fp32 nor the weight's dtype, ERR_UNSUPPORTED for operands that are not 16-byte aligned).
+// `a` / `y`: input and output forward, grad_output and grad_input transposed; `lin`: U forward, V transposed.
+static int lora_checks(const aqlm_b200_weight_t* w, const aqlm_b200_lora_t* lora, const void* a, const void* lin, void* y,
+                       int64_t batch, bool transposed, const char* what) {
+  int rc = validate(w, true);
+  if (rc) return rc;
+  if (batch < 0) return fail(AQLM_B200_ERR_SHAPE, "%s: negative batch", what);
+  if (!a || !y) return fail(AQLM_B200_ERR_SHAPE, "%s: input/output pointer is NULL", what);
+  if (!lora) return fail(AQLM_B200_ERR_SHAPE, "%s: adapter descriptor is NULL", what);
+  const void* aw = transposed ? lora->down : lora->up;
+  if (!aw || !lin) return fail(AQLM_B200_ERR_SHAPE, "%s: adapter %s or %s pointer is NULL", what,
+                               transposed ? "down" : "up", transposed ? "V" : "U");
+  if (lora->rank < 8 || lora->rank > 64 || lora->rank % 8 != 0)
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s: adapter rank must be a multiple of 8 in [8, 64], got %d", what, lora->rank);
+  if (lora->dtype != AQLM_B200_F32 && lora->dtype != w->dtype)
+    return fail(AQLM_B200_ERR_DTYPE, "%s: adapter operands must be fp32 or the weight's dtype, got dtype %d", what,
+                lora->dtype);
+  if (((reinterpret_cast<uintptr_t>(aw) | reinterpret_cast<uintptr_t>(lin)) & 15) != 0)
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s: adapter operands must be 16-byte aligned", what);
+  return AQLM_B200_OK;
+}
+
+// One adapter call of the wgmma GEMM (forward or transposed): checks, then one launch.  There is no GEMV form: a layout
+// the kernel does not take is ERR_UNSUPPORTED.
+static int lora_gemm(const aqlm_b200_weight_t* w, const aqlm_b200_lora_t* lora, const void* a, const void* lin, void* y,
+                     int64_t batch, bool transposed, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* what = transposed ? "LoRA transposed GEMM" : "LoRA GEMM";
+  int rc = lora_checks(w, lora, a, lin, y, batch, transposed, what);
+  if (rc || (rc = gemm_layout_checks(w, a, transposed, what)) || batch == 0) return rc;
+  GemmCall c = plain_gemm_call(w, a, y, batch, transposed, false);
+  c.lora = lora;
+  c.lora_in = lin;
+  if ((rc = run_gemm(c, workspace, workspace_bytes, stream)) != kNoGemmPlan) return rc;
+  return fail(AQLM_B200_ERR_UNSUPPORTED, "%s: no wgmma plan for this descriptor and batch", what);
 }
 
 // ---- fused weight-gradient GEMM: host side ------------------------------------------------------------------------
@@ -901,6 +956,45 @@ int aqlm_b200_matmat_grouped(const aqlm_b200_weight_t* w, const int64_t* seg_row
       return fail(AQLM_B200_ERR_UNSUPPORTED, "grouped launch: activation tile does not fit in shared memory");
     return with_dtype(w->dtype, [&](auto tag) { return launch_1x16<typename decltype(tag)::type, BT>(p, di, st); });
   });
+}
+
+int aqlm_b200_matmat_lora(const aqlm_b200_weight_t* w, const aqlm_b200_lora_t* lora, const void* input, const void* lora_in,
+                          void* output, int64_t batch, void* stream) {
+  const char* what = "LoRA GEMV";
+  int rc = lora_checks(w, lora, input, lora_in, output, batch, false, what);
+  if (rc) return rc;
+  if (w->num_codebooks != 1 || w->nbits_per_codebook != 16 || w->in_group_size != 8)
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s is implemented for the 1x16 (in_group 8) scheme only", what);
+  if (batch > 8) return fail(AQLM_B200_ERR_UNSUPPORTED, "%s takes at most 8 batch rows, got %lld", what, (long long)batch);
+  const size_t row_bytes = (size_t)(w->in_features / 8) * 2;
+  if (row_bytes % 16 != 0 || (reinterpret_cast<uintptr_t>(w->codes) & 15) || (reinterpret_cast<uintptr_t>(input) & 15))
+    return fail(AQLM_B200_ERR_UNSUPPORTED, "%s needs 16-byte aligned code rows and input", what);
+  if (batch == 0) return AQLM_B200_OK;
+  const DeviceInfo* di;
+  if ((rc = current_device(&di))) return rc;
+  const GemvParams p = gemv_params(w, input, output, batch, false);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return with_batch_tile(batch, [&](auto BT) {
+    const size_t smem = vec_smem_bytes(p, 1, 2, 8, BT, false, di->sm_count);
+    if (smem > (size_t)di->max_smem_optin - 1024)
+      return fail(AQLM_B200_ERR_UNSUPPORTED, "%s: activation tile does not fit in shared memory", what);
+    return with_dtype(w->dtype, [&](auto tag) {
+      return launch<gemv_1x16_lora_kernel<typename decltype(tag)::type, BT>>(di, di->sm_count, kGemv1x16Threads, smem, st,
+                                                                              0, p, lora_args(lora, lora_in, false));
+    });
+  });
+}
+
+int aqlm_b200_matmat_dequant_lora(const aqlm_b200_weight_t* w, const aqlm_b200_lora_t* lora, const void* input,
+                                  const void* lora_in, void* output, int64_t batch, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+  return lora_gemm(w, lora, input, lora_in, output, batch, false, workspace, workspace_bytes, stream);
+}
+
+int aqlm_b200_matmat_dequant_transposed_lora(const aqlm_b200_weight_t* w, const aqlm_b200_lora_t* lora,
+                                             const void* grad_output, const void* lora_in, void* grad_input,
+                                             int64_t batch, void* workspace, size_t workspace_bytes, void* stream) {
+  return lora_gemm(w, lora, grad_output, lora_in, grad_input, batch, true, workspace, workspace_bytes, stream);
 }
 
 int aqlm_b200_matmat(const aqlm_b200_weight_t* w, const void* input, void* output, int64_t batch, void* stream) {

@@ -163,6 +163,35 @@ __device__ __forceinline__ float dot8f(const float* w, const uint4& x, float acc
   return acc;
 }
 
+// LoRA adapter of a linear, as the fused kernels take it (aqlm_b200_lora_t on the device side).  The kernel adds
+// scaling * sum_j lin[t][j] * w(m, j), summed in fp32, to output element (t, m) before its one rounding to T:
+//   forward:    lin = U = dropout(x) . A^T [batch][rank],  w(o, j) = B[o][j]   (B = up,   [out][rank])
+//   transposed: lin = V = grad_out . B     [batch][rank],  w(i, j) = A[j][i]   (A = down, [rank][in])
+// All of it is read after griddep_wait(): lin comes from the previous kernel, A and B from the optimizer step.
+struct LoraArgs {
+  const void* lin;
+  const void* w;
+  int rank;     // 8..64, a multiple of 8
+  int f32;      // 1: adapter operands are fp32, 0: T
+  float scaling;
+};
+
+// Elements idx .. idx + 3 (idx % 4 == 0, 16-byte aligned rows) of an adapter operand, as fp32
+template <typename T>
+__device__ __forceinline__ float4 lora_load4(const void* base, size_t idx, int f32) {
+  if (f32) return *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(base) + idx);
+  const uint2 v = *reinterpret_cast<const uint2*>(reinterpret_cast<const T*>(base) + idx);
+  const float2 a = DT<T>::unpack2(v.x), b = DT<T>::unpack2(v.y);
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+
+__device__ __forceinline__ float dot4(const float4& a, const float4& b, float acc) {
+  acc = fmaf(a.x, b.x, acc);
+  acc = fmaf(a.y, b.y, acc);
+  acc = fmaf(a.z, b.z, acc);
+  return fmaf(a.w, b.w, acc);
+}
+
 // Extract element `idx` (compile-time after unrolling) of CODE_BYTES-wide unsigned codes from a 16-byte chunk.
 template <int CODE_BYTES>
 __device__ __forceinline__ uint32_t chunk_code(const uint4& c, int idx) {

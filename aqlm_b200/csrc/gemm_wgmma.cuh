@@ -112,13 +112,78 @@ __host__ __device__ inline GemmSmem gemm_smem_layout(int stages, int n_tile, int
   return L;
 }
 
+// The LoRA term of one tile (LoraArgs), staged in fp32 in the pipeline's shared memory once the main loop has drained
+// it (stage buffers and code tiles: everything below the barriers, which the plan always has room for,
+// gemm_lora_smem_bytes): ws = the weight side w(m, j) of the tile's 128 rows, us = lin of its N batch rows, each row
+// ld = rank + 4 floats apart (an odd number of 16-byte chunks: float4 reads of 8 consecutive rows are conflict-free).
+// Rows past the tile's end are staged as zeros.
+__host__ __device__ inline size_t gemm_lora_smem_bytes(int rank, int n_tile) {
+  return (size_t)(kGemmBlockM + n_tile) * (rank + 4) * 4;
+}
+
+struct GemmLoraTile {
+  LoraArgs a;
+  float* ws;
+  float* us;
+  int ld;
+
+  // Every thread tid < nthreads of the caller's group takes part; the caller synchronises the group afterwards.
+  // Forward: w(m, j) = B[m0 + m][j], rows of B.  Transposed: w(m, j) = A[j][m0 + m], columns of A (m_size = in, a
+  // multiple of 8, so 4 consecutive columns are one aligned load).  us: lin rows n0 .. n0 + n_tile - 1.
+  template <typename T, bool TRANSPOSED>
+  __device__ __forceinline__ void stage(int m0, int rows, int m_size, int n0, int ncols, int n_tile, int tid,
+                                        int nthreads) const {
+    const int q4 = a.rank >> 2;
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    if constexpr (TRANSPOSED) {
+      for (int i = tid; i < a.rank * (kGemmBlockM / 4); i += nthreads) {
+        const int j = i / (kGemmBlockM / 4), m = 4 * (i % (kGemmBlockM / 4));
+        const float4 v = m < rows ? lora_load4<T>(a.w, (size_t)j * m_size + m0 + m, a.f32) : zero;
+        ws[(m + 0) * ld + j] = v.x;
+        ws[(m + 1) * ld + j] = v.y;
+        ws[(m + 2) * ld + j] = v.z;
+        ws[(m + 3) * ld + j] = v.w;
+      }
+    } else {
+      for (int i = tid; i < kGemmBlockM * q4; i += nthreads) {
+        const int m = i / q4, q = i % q4;
+        *reinterpret_cast<float4*>(ws + m * ld + 4 * q) =
+            m < rows ? lora_load4<T>(a.w, (size_t)(m0 + m) * a.rank + 4 * q, a.f32) : zero;
+      }
+    }
+    for (int i = tid; i < n_tile * q4; i += nthreads) {
+      const int c = i / q4, q = i % q4;
+      *reinterpret_cast<float4*>(us + c * ld + 4 * q) =
+          c < ncols ? lora_load4<T>(a.lin, (size_t)(n0 + c) * a.rank + 4 * q, a.f32) : zero;
+    }
+  }
+
+  // scaling * L for tile row m and the 4 columns c0 + u * step (columns past the staged ones read the last staged one;
+  // the caller discards them)
+  __device__ __forceinline__ void cols4(int m, int c0, int step, int ncols, float (&out)[4]) const {
+    float l[4] = {0.f, 0.f, 0.f, 0.f};
+    const float* w = ws + m * ld;
+    const float* u[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) u[k] = us + min(c0 + k * step, ncols - 1) * ld;
+    for (int q = 0; q < a.rank; q += 4) {
+      const float4 wv = *reinterpret_cast<const float4*>(w + q);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) l[k] = dot4(wv, *reinterpret_cast<const float4*>(u[k] + q), l[k]);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) out[k] = __fmul_rn(a.scaling, l[k]);
+  }
+};
+
 // Split-K fix-up shared by both GEMM kernels: the LAST-arriving split of a tile adds all partials in split order
 // (deterministic) with the whole CTA; partials are [split][column][128 rows].  Writes y[n * ld + row0 + r] =
 // v * scale[row] + bias[row] (scales == nullptr: no scale / bias); an fp32 output (OutT = float) gets the sum v itself.
-template <typename T, typename OutT = T>
+// LORA: the last CTA stages the tile's LoRA term (lt, direction TRANSPOSED) and adds it before the rounding.
+template <typename T, typename OutT = T, bool LORA = false, bool TRANSPOSED = false>
 __device__ __forceinline__ void gemm_splitk_fixup(uint32_t* flag, unsigned int* counter, const float* parts, int ksplit, int N,
                                                   int ncols, OutT* y, long long ld, int n0, int row0, int rows,
-                                                  const T* scales, const T* bias) {
+                                                  const T* scales, const T* bias, const GemmLoraTile* lt = nullptr) {
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -128,6 +193,10 @@ __device__ __forceinline__ void gemm_splitk_fixup(uint32_t* flag, unsigned int* 
     if (last) *counter = 0u;  // leave the counter clean for the next call
   }
   __syncthreads();
+  if constexpr (LORA) {
+    if (*flag) lt->stage<T, TRANSPOSED>(row0, rows, (int)ld, n0, ncols, N, threadIdx.x, kGemmThreads);
+    __syncthreads();
+  }
   constexpr int kPhases = kGemmThreads / kGemmBlockM;  // column phases of 128 threads each
   if (*flag && threadIdx.x < kPhases * kGemmBlockM) {
     __threadfence();
@@ -146,11 +215,14 @@ __device__ __forceinline__ void gemm_splitk_fixup(uint32_t* flag, unsigned int* 
             if (cc < ncols) v[u] += __ldcg(parts + ((size_t)sp * N + cc) * kGemmBlockM + rrow);
           }
         }
+float l[4];
+        if constexpr (LORA) lt->cols4(rrow, c, kPhases, ncols, l);
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
           const int cc = c + u * kPhases;
           if (cc >= ncols) continue;
           if constexpr (std::is_same<OutT, float>::value) y[(size_t)(n0 + cc) * ld + row] = v[u];
+          else if constexpr (LORA) y[(size_t)(n0 + cc) * ld + row] = DT<T>::from_float(__fadd_rn(fmaf(v[u], sc, bi), l[u]));
           else y[(size_t)(n0 + cc) * ld + row] = DT<T>::from_float(fmaf(v[u], sc, bi));
         }
       }
@@ -179,6 +251,7 @@ struct GemmForward {
 
   // Scale (and bias) are applied to the sums in the epilogue / the split-K fix-up; tiles may be ragged (tile_m < 128).
   static constexpr bool kScaleInProducer = false;
+  static constexpr bool kTransposed = false;
   static __device__ __forceinline__ int tile_m(const GemmParams& p) { return p.tile_m; }
   // out rows of one expert of a routed call (the forward's output rows)
   static __device__ __forceinline__ int out_rows(const GemmParams& p) { return p.m_size; }
@@ -214,10 +287,14 @@ struct GemmForward {
 // The pipeline of both GEMM kernels; Dir is GemmForward or GemmTransposed, N the MMA width (columns of the batch tile).
 // tmap_b loads the K-major B operand (activations / grad_output), tmap_codes the code tiles.  GROUPED: the kernel of
 // grouped calls (GemmParams::n_seg / seg_end); plain linears run kernels without any segment arithmetic.  ROUTED (with
-// GROUPED): the kernel of routed calls (GemmParams::expert_off / n_experts); see the file comment.
-template <typename T, int N, typename Dir, bool GROUPED = false, bool ROUTED = false>
-__device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const CUtensorMap& tmap_codes, const GemmParams& p) {
+// GROUPED): the kernel of routed calls (GemmParams::expert_off / n_experts); see the file comment.  LORA (plain linears
+// only): the epilogue and the split-K fix-up add the LoRA term of `lora` (see LoraArgs) to every output element before
+// its rounding, staged over the drained pipeline (GemmLoraTile).
+template <typename T, int N, typename Dir, bool GROUPED = false, bool ROUTED = false, bool LORA = false>
+__device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const CUtensorMap& tmap_codes, const GemmParams& p,
+                                              const LoraArgs& lora = LoraArgs{}) {
   static_assert(!ROUTED || GROUPED, "a routed kernel resolves segments too");
+  static_assert(!LORA || !GROUPED, "an adapter belongs to one plain linear");
   constexpr int K = Dir::K, CODE_BYTES = Dir::CODE_BYTES, CB4 = Dir::CB4;
   constexpr int KB_PER_CTILE = Dir::kKbPerCtile;  // k-blocks covered by one code tile
   static_assert(KB_PER_CTILE >= 1, "scheme too wide for the code tile");
@@ -312,6 +389,56 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
       if (lane == 0) mbar_arrive(empty_bar(prev));
     }
     griddep_wait();  // before any global write (y, split-K partials): the previous kernel has completed
+    if constexpr (LORA) {
+      if (p.ksplit == 1) {
+        // both warpgroups' MMAs have completed, so every stage is drained: stage the tile's LoRA term over them
+        constexpr int kConsumerThreads = kGemmConsumerWarps * 32;
+        const int ld = lora.rank + 4;
+        const GemmLoraTile lt{lora, reinterpret_cast<float*>(gbase + L.a), reinterpret_cast<float*>(gbase + L.a) + kGemmBlockM * ld, ld};
+        asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
+        lt.stage<T, Dir::kTransposed>(m0, min(TM, p.m_size - m0), p.m_size, n0, min(N, n_end() - n0), N, threadIdx.x,
+                                      kConsumerThreads);
+        asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // the thread's tile rows: r0 and r0 + 8
+        float sc[2] = {1.f, 1.f}, bi[2] = {0.f, 0.f};
+        bool ok[2];
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const int row = m0 + r0 + 8 * j;
+          ok[j] = r0 + 8 * j < TM && row < p.m_size;
+          if (!Dir::kScaleInProducer && ok[j]) {
+            sc[j] = DT<T>::to_float(reinterpret_cast<const T*>(p.scales)[row]);
+            if (p.bias) bi[j] = DT<T>::to_float(reinterpret_cast<const T*>(p.bias)[row]);
+          }
+        }
+#pragma unroll
+        for (int i = 0; i < N / 8; ++i) {
+          const int col0 = 8 * i + 2 * (lane & 3);
+          const float* w0 = lt.ws + r0 * ld;
+          const float* u0 = lt.us + col0 * ld;
+          float l[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+          for (int q = 0; q < lora.rank; q += 4) {
+            const float4 a0 = *reinterpret_cast<const float4*>(w0 + q), a1 = *reinterpret_cast<const float4*>(w0 + 8 * ld + q);
+            const float4 b0 = *reinterpret_cast<const float4*>(u0 + q), b1 = *reinterpret_cast<const float4*>(u0 + ld + q);
+            l[0][0] = dot4(a0, b0, l[0][0]);
+            l[0][1] = dot4(a0, b1, l[0][1]);
+            l[1][0] = dot4(a1, b0, l[1][0]);
+            l[1][1] = dot4(a1, b1, l[1][1]);
+          }
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+              if (!ok[j] || n0 + col0 + c >= n_end()) continue;
+              const float v = acc[4 * i + 2 * j + c], t = __fmul_rn(lora.scaling, l[j][c]);
+              y[(size_t)(n0 + col0 + c) * p.m_size + m0 + r0 + 8 * j] =
+                  DT<T>::from_float(Dir::kScaleInProducer ? __fadd_rn(v, t) : __fadd_rn(fmaf(v, sc[j], bi[j]), t));
+            }
+          }
+        }
+        return;  // without a split nothing follows the roles
+      }
+    }
     // accumulator fragment: register 4i + 2j + c holds (row 16 (warp % 4) + lane / 4 + 8 j, column 8 i + 2 (lane % 4) + c)
     float* my_part = p.ws_partials ? p.ws_partials + ((tile_id * p.ksplit + split) * (size_t)N) * kGemmBlockM : nullptr;
 #pragma unroll
@@ -530,7 +657,13 @@ __device__ __forceinline__ void gemm_pipeline(const CUtensorMap& tmap_b, const C
     uint32_t* flag = reinterpret_cast<uint32_t*>(gbase + L.flag);
     const float* parts = p.ws_partials + (tile_id * p.ksplit) * (size_t)N * kGemmBlockM;
     const int ncols = min(N, n_end() - n0), rows = min(TM, p.m_size - m0);
-    if constexpr (Dir::kScaleInProducer) {
+    if constexpr (LORA) {
+      const int ld = lora.rank + 4;
+      const GemmLoraTile lt{lora, reinterpret_cast<float*>(gbase + L.a), reinterpret_cast<float*>(gbase + L.a) + kGemmBlockM * ld, ld};
+      gemm_splitk_fixup<T, T, true, Dir::kTransposed>(flag, p.ws_counters + tile_id, parts, p.ksplit, N, ncols, y, p.m_size,
+                                                      n0, m0, rows, Dir::kScaleInProducer ? nullptr : reinterpret_cast<const T*>(p.scales),
+                                                      Dir::kScaleInProducer ? nullptr : reinterpret_cast<const T*>(p.bias), &lt);
+    } else if constexpr (Dir::kScaleInProducer) {
       gemm_splitk_fixup<T>(flag, p.ws_counters + tile_id, parts, p.ksplit, N, ncols, y, p.m_size, n0, m0, rows, nullptr, nullptr);
     } else {
       if (p.partial_f32)
@@ -561,6 +694,14 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_dequant_grouped_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_codes,
                             const GemmParams p) {
   gemm_pipeline<T, N, GemmForward<K, CODE_BYTES>, true>(tmap_x, tmap_codes, p);
+}
+
+// A plain linear with a LoRA adapter (LoraArgs, forward form): y = x W^T s + b + scaling (x A^T) B^T, one rounding.
+template <typename T, int K, int CODE_BYTES, int N>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_dequant_lora_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_codes,
+                         const GemmParams p, const LoraArgs lora) {
+  gemm_pipeline<T, N, GemmForward<K, CODE_BYTES>, false, false, true>(tmap_x, tmap_codes, p, lora);
 }
 
 // A routed call: every expert of a mixture-of-experts projection in one launch, over expert-sorted input rows.

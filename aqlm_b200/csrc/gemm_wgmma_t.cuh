@@ -40,6 +40,7 @@ struct GemmTransposed {
 
   // The producer multiplies every vector by the scale of its out row; the epilogue and the fix-up only cast.
   static constexpr bool kScaleInProducer = true;
+  static constexpr bool kTransposed = true;
   static __device__ __forceinline__ int tile_m(const GemmParams&) { return kGemmBlockM; }
   // out rows of one expert of a routed call (the contraction's length)
   static __device__ __forceinline__ int out_rows(const GemmParams& p) { return p.k_size; }
@@ -78,6 +79,15 @@ template <typename T, int K, int CODE_BYTES, int N>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_dequant_t_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_constant__ CUtensorMap tmap_codes, const GemmParams p) {
   gemm_pipeline<T, N, GemmTransposed<K, CODE_BYTES>>(tmap_g, tmap_codes, p);
+}
+
+// The backward of a plain linear with a LoRA adapter (LoraArgs, transposed form): grad_in = (grad_out s) W + scaling V A,
+// V = grad_out . B computed by the caller, one rounding.
+template <typename T, int K, int CODE_BYTES, int N>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_dequant_t_lora_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_constant__ CUtensorMap tmap_codes,
+                           const GemmParams p, const LoraArgs lora) {
+  gemm_pipeline<T, N, GemmTransposed<K, CODE_BYTES>, false, false, true>(tmap_g, tmap_codes, p, lora);
 }
 
 // The backward of a grouped call: grad_output holds the members' output gradients side by side.

@@ -225,8 +225,11 @@ constexpr int kGemv1x16Threads = 512;
 //   fence, flag or barrier in between (see the epilogue).  A thread only ever waits for the same element of the other ranks.
 // Two buffer sets alternate by step parity; `step` is read after griddepcontrol.wait (the previous launch, which
 // advances it, has completed).  The grid is one CTA per SM, all co-resident, so the cross-rank wait cannot deadlock.
-template <typename T, int BT, bool PEER = false>
-__global__ void __launch_bounds__(kGemv1x16Threads, 1) gemv_1x16_kernel(const GemvParams p, const GemvPeer pc) {
+// LORA (not with PEER): the epilogue adds a LoRA adapter's up-projection (LoraArgs, forward form) to every output
+// element before its rounding; the adapter's U row and B row are read from global memory (L1) after griddep_wait().
+template <typename T, int BT, bool PEER, bool LORA>
+__device__ __forceinline__ void gemv_1x16(const GemvParams& p, const GemvPeer& pc, const LoraArgs& lora) {
+  static_assert(!(PEER && LORA), "the fused exchange has no adapter term");
   extern __shared__ __align__(16) uint8_t smem_raw[];
   constexpr int THREADS = kGemv1x16Threads;
   constexpr int kWarps = THREADS / 32;
@@ -336,7 +339,16 @@ __global__ void __launch_bounds__(kGemv1x16Threads, 1) gemv_1x16_kernel(const Ge
       const int row = row_first + ri * row_step;
       float v = 0.f;
       for (int sl = 0; sl < slices; ++sl) v += spart[((size_t)ri * slices + sl) * BT + b];
-      if (p.partial_f32) {
+      if constexpr (LORA) {
+        float l = 0.f;
+        for (int j = 0; j < lora.rank; j += 4)
+          l = dot4(lora_load4<T>(lora.lin, (size_t)b * lora.rank + j, lora.f32),
+                   lora_load4<T>(lora.w, (size_t)row * lora.rank + j, lora.f32), l);
+        const float s = DT<T>::to_float(reinterpret_cast<const T*>(p.scales)[row]);
+        const float bv = p.bias ? DT<T>::to_float(reinterpret_cast<const T*>(p.bias)[row]) : 0.f;
+        reinterpret_cast<T*>(p.y)[(size_t)b * p.out_features + row] =
+            DT<T>::from_float(__fadd_rn(fmaf(v, s, bv), __fmul_rn(lora.scaling, l)));
+      } else if (p.partial_f32) {
         reinterpret_cast<float*>(p.y)[(size_t)b * p.out_features + row] = v;
       } else {
         const float s = DT<T>::to_float(reinterpret_cast<const T*>(p.scales)[row]);
@@ -396,6 +408,17 @@ __global__ void __launch_bounds__(kGemv1x16Threads, 1) gemv_1x16_kernel(const Ge
       }
     }
   }
+}
+
+template <typename T, int BT, bool PEER = false>
+__global__ void __launch_bounds__(kGemv1x16Threads, 1) gemv_1x16_kernel(const GemvParams p, const GemvPeer pc) {
+  gemv_1x16<T, BT, PEER, false>(p, pc, LoraArgs{});
+}
+
+// A plain 1x16 linear with a LoRA adapter (rows dealt round-robin, no partials).
+template <typename T, int BT>
+__global__ void __launch_bounds__(kGemv1x16Threads, 1) gemv_1x16_lora_kernel(const GemvParams p, const LoraArgs lora) {
+  gemv_1x16<T, BT, false, true>(p, GemvPeer{}, lora);
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -523,6 +523,86 @@ def matmat_dequant_transposed(input, codes, codebooks, scales, bias=None) -> tor
     return out.reshape(input.shape[:-1] + (w.in_features,))
 
 
+# ---- LoRA adapters fused into the base kernels (csrc: gemv_1x16_lora_kernel, gemm_dequant[_t]_lora_kernel) --------
+def _lora(lin, weight, scaling: float, device, w, transposed: bool):
+    """The adapter descriptor of one call and `lin` as a contiguous 2-D tensor, or None when the operands are not what
+    the kernels take (one dtype, fp32 or the weight's).  `weight` is B [out, rank] forward, A [rank, in] transposed."""
+    rank = weight.shape[0] if transposed else weight.shape[1]
+    expect = (rank, w.in_features) if transposed else (w.out_features, rank)
+    if weight.dim() != 2 or tuple(weight.shape) != expect or lin.shape[-1] != rank:
+        raise ValueError(f"adapter shapes: lin {tuple(lin.shape)}, {'down' if transposed else 'up'} "
+                         f"{tuple(weight.shape)}, expected {expect}")
+    _require_cuda(lin, weight)
+    if lin.device != device or weight.device != device:
+        raise ValueError("adapter operands must be on the weight's device")
+    if lin.dtype != weight.dtype or lin.dtype not in (torch.float32, _dtype_torch(w.dtype)):
+        return None, None, None
+    d = _cabi.Lora()
+    d.down = weight.data_ptr() if transposed else None
+    d.up = None if transposed else weight.data_ptr()
+    d.rank = rank
+    d.dtype = _cabi.F32 if lin.dtype == torch.float32 else w.dtype
+    d.scaling = float(scaling)
+    flat = lin.reshape(-1, rank)
+    return d, flat if flat.is_contiguous() else flat.contiguous(), weight if weight.is_contiguous() else None
+
+
+def _dtype_torch(code: int) -> torch.dtype:
+    return torch.float16 if code == _cabi.F16 else torch.bfloat16
+
+
+def _lora_call(a, codes, codebooks, scales, bias, lin, weight, scaling, transposed: bool, gemv: bool):
+    device, w, flat = _operands(a, codes, codebooks, scales, None if transposed else bias, transposed)
+    d, flat_lin, weight = _lora(lin, weight, scaling, device, w, transposed)
+    if d is None or weight is None:
+        return None
+    if flat_lin.shape[0] != flat.shape[0]:
+        raise ValueError(f"adapter input has {flat_lin.shape[0]} rows, the call {flat.shape[0]}")
+    batch = flat.shape[0]
+    n_out = w.in_features if transposed else w.out_features
+    out = torch.empty((batch, n_out), dtype=a.dtype, device=device)
+    wp, lp = ctypes.byref(w), ctypes.byref(d)
+    args = (wp, lp, flat.data_ptr(), flat_lin.data_ptr(), out.data_ptr(), batch)
+    if gemv:
+        with _on_device(device):
+            rc = _cabi.lib().aqlm_b200_matmat_lora(*args, _stream_ptr(device))
+        ok = rc != _cabi.ERR_UNSUPPORTED
+        _cabi.check(rc if ok else _cabi.OK)
+    elif transposed:
+        ok = _call(device, "aqlm_b200_matmat_dequant_transposed_workspace_bytes", (wp, batch),
+                   "aqlm_b200_matmat_dequant_transposed_lora", args)
+    else:
+        ok = _call(device, "aqlm_b200_matmat_dequant_workspace_bytes", (wp, batch), "aqlm_b200_matmat_dequant_lora", args)
+    return out.reshape(a.shape[:-1] + (n_out,)) if ok else None
+
+
+def matmat_lora(input, codes, codebooks, scales, bias, lora_u, lora_up, scaling: float) -> Optional[torch.Tensor]:
+    """A 1x16 linear with a LoRA adapter at up to 8 rows, in ONE GEMV launch: base(input) + scaling * lora_u @ lora_up^T,
+    added in fp32 before the output's one rounding.  `lora_u` = dropout(input) @ A^T [..., rank], `lora_up` = B [out,
+    rank], both fp32 or both the weight's dtype.  None when the library does not take the call (another scheme, more rows,
+    a rank outside 8..64 or not a multiple of 8, misaligned operands, another adapter dtype)."""
+    return _lora_call(input, codes, codebooks, scales, bias, lora_u, lora_up, scaling, False, True)
+
+
+def matmat_dequant_lora(input, codes, codebooks, scales, bias, lora_u, lora_up, scaling: float) -> Optional[torch.Tensor]:
+    """`matmat_lora` at any batch in ONE wgmma GEMM launch, for every scheme the GEMM takes.  None as for matmat_lora."""
+    return _lora_call(input, codes, codebooks, scales, bias, lora_u, lora_up, scaling, False, False)
+
+
+def matmat_dequant_transposed_lora(grad_out, codes, codebooks, scales, lora_v, lora_down,
+                                   scaling: float) -> Optional[torch.Tensor]:
+    """Backward w.r.t. the input of a linear with a LoRA adapter (dropout inactive) in ONE transposed wgmma GEMM launch:
+    (grad_out * scales) @ W + scaling * lora_v @ lora_down, `lora_v` = grad_out @ B [..., rank], `lora_down` = A [rank,
+    in].  None when the library does not take the call (see matmat_lora)."""
+    return _lora_call(grad_out, codes, codebooks, scales, None, lora_v, lora_down, scaling, True, False)
+
+
+def _or_unsupported(y):
+    if y is None:
+        raise NotImplementedError("aqlm_b200: no fused LoRA kernel takes this layout or adapter")
+    return y
+
+
 # ---- torch.library registration (reference cuda_kernel.py:13-132) ---------------------------------------
 _SCHEMA = "(Tensor input, Tensor codes, Tensor codebooks, Tensor scales, Tensor? bias) -> Tensor"
 _LIB = torch.library.Library("aqlm", "FRAGMENT")
@@ -541,9 +621,9 @@ def _cpu_refusal(*args, **kwargs):
     raise NotImplementedError("aqlm_b200 ops run on CUDA (sm_90a) only; there is no CPU fallback in this package")
 
 
-def _register(name: str, fn, fake) -> None:
+def _register(name: str, fn, fake, schema: str = _SCHEMA) -> None:
     qual = f"aqlm::{name}"
-    _LIB.define(f"{name}{_SCHEMA}")
+    _LIB.define(f"{name}{schema}")
     _LIB.impl(name, fn, "CUDA")
     _LIB.impl(name, _cpu_refusal, "CPU")
     torch.library.register_fake(qual, fake, lib=_LIB)
@@ -555,6 +635,27 @@ for _scheme in ("code1x16", "code2x8", "code1x8", "generic"):
     _register(f"{_scheme}_matmat_dequant", matmat_dequant, _fake_forward)
     _register(f"{_scheme}_matmat_dequant_transposed", matmat_dequant_transposed, _fake_transposed)
     OP_NAMES += [f"{_scheme}_matmat", f"{_scheme}_matmat_dequant", f"{_scheme}_matmat_dequant_transposed"]
+
+# LoRA ops: the adapter's rank-sized product (U, or V in the backward) and B (or A) join the base operands.  The ops
+# raise NotImplementedError where the Python functions above return None.
+_LORA_SCHEMA = ("(Tensor input, Tensor codes, Tensor codebooks, Tensor scales, Tensor? bias, Tensor lora_in, "
+                "Tensor lora_weight, float scaling) -> Tensor")
+
+
+def _fake_lora_forward(input, codes, codebooks, scales, bias, lora_in, lora_weight, scaling):
+    return _fake_forward(input, codes, codebooks, scales)
+
+
+def _fake_lora_transposed(input, codes, codebooks, scales, bias, lora_in, lora_weight, scaling):
+    return _fake_transposed(input, codes, codebooks, scales)
+
+
+_register("lora_matmat", lambda *a: _or_unsupported(matmat_lora(*a)), _fake_lora_forward, _LORA_SCHEMA)
+_register("lora_matmat_dequant", lambda *a: _or_unsupported(matmat_dequant_lora(*a)), _fake_lora_forward, _LORA_SCHEMA)
+_register("lora_matmat_dequant_transposed",
+          lambda x, c, cb, s, b, v, a, sc: _or_unsupported(matmat_dequant_transposed_lora(x, c, cb, s, v, a, sc)),
+          _fake_lora_transposed, _LORA_SCHEMA)
+OP_NAMES += ["lora_matmat", "lora_matmat_dequant", "lora_matmat_dequant_transposed"]
 
 # The functions the reference's pybind module exports (cuda_kernel.cpp:686-699).
 CUDA_KERNEL = SimpleNamespace(

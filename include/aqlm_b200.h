@@ -15,7 +15,9 @@
  * read before that kernel is known to be complete.  tests/test_zz_ordering.py launches each of these entry points
  * right behind an in-place kernel that rewrote one of its operands, with PDL on and off, and checks every output
  * exactly; it shows what was observed on the hardware it ran on, not a guarantee of the programming model.
- * Activations, expert offsets, workspaces and outputs are touched only after the wait.
+ * Activations, expert offsets, workspaces and outputs are touched only after the wait.  So is every operand of a LoRA
+ * adapter (aqlm_b200_*_lora): U or V comes from the previous kernel, and the adapter's A and B are rewritten by the
+ * optimizer step right before, so unlike codes and codebooks they are never read in the prologue.
  *
  * Host threads: the per-device queries and the per-kernel shared-memory attributes are set up under locks, so calls
  * may come from several host threads at once.  Calls that may run concurrently must not share a workspace.
@@ -51,7 +53,7 @@ typedef enum {
   AQLM_B200_ERR_ARCH = 5         /* device is not sm_90 -> RuntimeError */
 } aqlm_b200_status;
 
-typedef enum { AQLM_B200_F16 = 0, AQLM_B200_BF16 = 1 } aqlm_b200_dtype;
+typedef enum { AQLM_B200_F16 = 0, AQLM_B200_BF16 = 1, AQLM_B200_F32 = 2 /* LoRA adapter operands only */ } aqlm_b200_dtype;
 
 /* flags for aqlm_b200_matmat_ex, aqlm_b200_matmat_ws and aqlm_b200_matmat_dequant_ex */
 #define AQLM_B200_FLAG_PARTIAL_F32 1u /* write UNSCALED fp32 partial sums (no scale, no bias): the per-rank
@@ -95,6 +97,11 @@ void aqlm_b200_reload_tunables(void);
  *   aqlm_b200_dequant: rT(rf32(s * Wsum)), or rT(Wsum) without scales
  *   aqlm_b200_scale_bias, aqlm_b200_allreduce_scale_bias: rT(rf32(p * s + b))
  *   aqlm_b200_matmat_weight_grad: grad_scales from rT(Wsum), the operand the wgmma forward multiplies
+ *   LoRA adapters (aqlm_b200_*_lora), with L = rf32(sum_j U[t][j] * B[o][j]) (forward) or rf32(sum_j V[t][j] * A[j][i])
+ *   (transposed), the adapter operands taken exactly as given (fp32, or T widened):
+ *       aqlm_b200_matmat_lora:           y = rT(rf32(rf32(sum_j x * Wsum * s + b) + rf32(scaling * L)))
+ *       aqlm_b200_matmat_dequant_lora:   y = rT(rf32(rf32(sum_j x * rT(Wsum) * s + b) + rf32(scaling * L)))
+ *       aqlm_b200_matmat_dequant_transposed_lora: grad_in = rT(rf32(sum_o g * rT(rf32(s * Wsum)) + rf32(scaling * L)))
  * So for K >= 2 the two forward families differ by the rounding of W: the same row of the same layer can come out
  * differently on either side of the GEMV / wgmma batch boundary.  For K = 1, Wsum is a codebook entry and both agree.
  * Subnormal f16 scales, inputs and outputs are kept (no flush to zero); an f16 output past 65504 is +-inf. */
@@ -252,6 +259,40 @@ int aqlm_b200_matmat_weight_grad_routed(const aqlm_b200_weight_t* w, const int64
                                         const int32_t* expert_offsets, const void* input, const void* grad_output,
                                         int64_t rows, float* grad_codebooks, float* grad_scales, void* workspace,
                                         size_t workspace_bytes, void* stream);
+
+/* ---- LoRA adapters on a plain linear: the adapter's up-projection fused into the base kernel's epilogue ----------
+ * PEFT's LoRA linear computes y = base(x) + scaling * (dropout(x) . A^T) . B^T with A = down [rank][in_features] and
+ * B = up [out_features][rank].  The caller computes the rank-sized product and the kernel adds the rest in the epilogue
+ * of the base GEMV or GEMM, summed in fp32 and added before the output's single rounding (see Rounding):
+ *   aqlm_b200_matmat_lora, aqlm_b200_matmat_dequant_lora:
+ *       output[t][o] = base(input)[t][o] + scaling * sum_j lora_in[t][j] * up[o][j]        lora_in = U [batch][rank]
+ *   aqlm_b200_matmat_dequant_transposed_lora (backward w.r.t. the input, dropout inactive):
+ *       grad_input[t][i] = (grad_output . diag(scales) . W)[t][i] + scaling * sum_j lora_in[t][j] * down[j][i]
+ *                                                                                   lora_in = V = grad_output . B
+ * Adapter operands (down, up, lora_in) are all fp32 (AQLM_B200_F32, PEFT's default) or all the weight's dtype, with
+ * 16-byte aligned rows: rank 8..64 and a multiple of 8.  aqlm_b200_matmat_lora takes the 1x16 (in_group 8) scheme, up
+ * to 8 batch rows, 16-byte aligned code rows and input; the GEMMs take the layouts of the grouped GEMMs (in_group 8,
+ * 8/16-bit codes, 1/2/4/8 codebooks, in_features % 64 == 0 forward, out_features % 8 == 0 transposed) and the
+ * workspace of aqlm_b200_matmat_dequant[_transposed]_workspace_bytes.  Anything else returns AQLM_B200_ERR_UNSUPPORTED
+ * (a rank out of range, misaligned operands, another scheme): there is no fallback with another rounding, the caller
+ * runs its own formulation.  A NULL descriptor or pointer is AQLM_B200_ERR_SHAPE, an adapter dtype that is neither
+ * fp32 nor the weight's AQLM_B200_ERR_DTYPE; all of these before any device query.  batch == 0: OK, no launch; exactly
+ * one launch otherwise.  Capturable. */
+typedef struct {
+  const void* down; /* A [rank][in_features] */
+  const void* up;   /* B [out_features][rank] */
+  int32_t rank;
+  int32_t dtype;    /* AQLM_B200_F32 or the weight's dtype */
+  float scaling;    /* lora_alpha / rank, or lora_alpha / sqrt(rank) (rsLoRA) */
+} aqlm_b200_lora_t;
+int aqlm_b200_matmat_lora(const aqlm_b200_weight_t* w, const aqlm_b200_lora_t* lora, const void* input, const void* lora_in,
+                          void* output, int64_t batch, void* stream);
+int aqlm_b200_matmat_dequant_lora(const aqlm_b200_weight_t* w, const aqlm_b200_lora_t* lora, const void* input,
+                                  const void* lora_in, void* output, int64_t batch, void* workspace,
+                                  size_t workspace_bytes, void* stream);
+int aqlm_b200_matmat_dequant_transposed_lora(const aqlm_b200_weight_t* w, const aqlm_b200_lora_t* lora,
+                                             const void* grad_output, const void* lora_in, void* grad_input,
+                                             int64_t batch, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Epilogue of the sharded path: output[b,o] = (T)(partial[b,o] * scales[o] + bias[o]) after the
  * all-reduce of the fp32 partials (new work; the reference has no multi-GPU hot path, SURVEY §8e). */
